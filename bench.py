@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200 Newton iteration core.
+"""bench.py — headline benchmark of the Newton iteration core on one H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--N 100]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--N 100] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[2], the configuration the metric is quoted on): 3D Brusselator N=100 (10^6 cells, 2*10^6
 unknowns), NewtonRaphson(linsolve = KrylovJL_GMRES()) with the matrix-free exact JVP, abstol = 1e-8 (the reference
@@ -25,6 +25,8 @@ BASELINE configuration, each with its own CPU baseline (rank 0 only, after the t
   `precond`    config 3 with the multigrid `precs` + EisenstatWalkerForcing2 (Arnoldi iterations, Newton steps/s);
   `ensemble`   config 5: 8192 x (2D N=32), sharded over the ranks, gathered through the library's C-ABI collective.
 `--impl reference` times the CPU restatement of the reference (oracle/, "port": the Julia reference cannot run here).
+`--dump-outputs DIR` writes what the last timed step returned to its caller — the root `u` and the residual `resid`, float64,
+2 x 16 MB at N = 100 — as DIR/u.npy and DIR/resid.npy; the inputs are synthetic and seeded, so two builds compare output for output.
 """
 import argparse
 import json
@@ -51,11 +53,11 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -352,7 +354,7 @@ def leg_lu(nls, torch, ctx):
     return {"workload": "bruss2d_N128_newtonraphson_dense_lu", "n": n, "jacobian_GB": 8.0 * n * n / 1e9, "fill_ms": fill_ms, "fill_gbs": 8.0 * n * n / (fill_ms * 1e-3) / 1e9,
             "getrf_s": t2 * 1e-3, "getrf_first_call_s": t1 * 1e-3, "lu_tflops": flops / (t2 * 1e-3) / 1e12, "getrs_ms": solve_ms, "solve_rel_residual": rel,
             "families_ms": {k: round(v["ms"], 2) for k, v in prof.items() if k.startswith("lu")},
-            "tensor_pipe": "trailing update on the FP64 tensor cores (DMMA); pipe utilisation from ncu: see profiles/README.md",
+            "tensor_pipe": "trailing update on the FP64 tensor cores (DMMA)",
             "cusolver_getrf_s": cs_ms * 1e-3, "cusolver_tflops": flops / (cs_ms * 1e-3) / 1e12, "vs_cusolver": cs_ms / t2, "pivots_equal_cusolver": same_pivots,
             "newton_solve_s": solve_s, "newton_nsteps": sol.stats.nsteps, "newton_nfactors": sol.stats.nfactors, "newton_resid_inf": sol.resid_inf,
             "newton_retcode": nls.ReturnCode.name(sol.retcode),
@@ -451,17 +453,6 @@ def leg_precond(nls, torch, ctx):
     return out
 
 
-def traffic_from_profile(bytes_per_launch, resident):
-    p = os.path.join(ROOT, "profiles", "r2_resident_traffic.json")
-    if resident and os.path.exists(p):
-        d = json.load(open(p))
-        ratio = d["dram_bytes"] / d["algorithmic_bytes"]
-        return {"traffic": bytes_per_launch * ratio,
-                "traffic_source": "ncu --set full, one launch: dram read+write %.4f GB vs %.4f GB algorithmic (ratio %.4f, %s) applied to this run's mean bytes per launch" % (
-                    d["dram_bytes"] / 1e9, d["algorithmic_bytes"] / 1e9, ratio, d["source"])}
-    return {"traffic": None, "traffic_source": "no ncu summary for this kernel under profiles/"}
-
-
 def run_b200(args):
     import numpy as np
     import torch
@@ -528,6 +519,10 @@ def run_b200(args):
     ctx.profile(False, reset=False)
     clk = clocks.stop() if rank == 0 else None
     assert sol.retcode == nls.ReturnCode.Success and sol.resid_inf < 1e-8, (sol.retcode, sol.resid_inf)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in (("u", sol.u), ("resid", sol.resid)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.asarray(arr.to_host(), dtype=np.float64))
     # ---- end-to-end timed region: host buffers, H2D + D2H inside
     barrier()
     e2, e3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -570,10 +565,6 @@ def run_b200(args):
     achieved = dom_bytes / (dom_ms * 1e-3) / 1e9 if dom_ms > 0 else 0.0
     roofline = {"bound": "hbm", "kernel": dom_name, "achieved": achieved, "peak": peak,
                 "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
-                # DRAM traffic cannot be counted from inside a plain run; it comes from the committed `ncu --set full` capture of this
-                # kernel (profiles/r2_resident_traffic.json, written by tools/ncu_traffic.py from the raw CSV): dram read + write
-                # bytes of ONE launch and the algorithmic bytes of that same launch.  Null when the summary is absent.
-                **traffic_from_profile(dom_bytes / max(dom_launches, 1), "resident" in dom),
                 "bytes_per_launch": dom_bytes / max(dom_launches, 1), "ms_per_launch": dom_ms / max(dom_launches, 1),
                 "share_of_step": dom_ms / (ms_local if ms_local > 0 else 1.0),
                 "whole_step_gbs": bytes_moved / (ms * 1e-3) / 1e9,
@@ -652,6 +643,8 @@ def main():
     ap.add_argument("--orth", default="mgs", choices=["mgs", "cgs2"], help="GMRES orthogonalisation: mgs = Krylov.jl default (reference), cgs2 = reorthogonalised")
     ap.add_argument("--no-ensemble", dest="no_ensemble", action="store_true", help="skip the config-5 ensemble leg")
     ap.add_argument("--no-legs", dest="no_legs", action="store_true", help="skip the n80 / lu / sparse_tr / precond legs (configs 2, 4 and the §8f variants)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="write the root and the residual of the last timed step as DIR/u.npy and DIR/resid.npy (float64)")
     args = ap.parse_args()
     with _OneLineStdout() as out:
         _OUT = out

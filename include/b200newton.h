@@ -1,5 +1,5 @@
 /*
- * b200newton.h — C ABI of libb200newton.so, the B200-native (sm_100a) Newton iteration core
+ * b200newton.h — C ABI of libb200newton.so, the H100-native (sm_90a) Newton iteration core
  * that sits behind NonlinearSolve.jl's first-order solver plugin points.
  *
  * Every entry point is `extern "C"`, takes plain pointers/sizes and returns an int32 status
@@ -150,7 +150,7 @@ typedef struct b200_gmres_opts {
   int32_t engine;     /* B200_ENGINE_* */
   int32_t check_every;/* host polls the device status every this many Arnoldi iterations (multi-kernel engine); 0 => 8 (2 with a preconditioner) */
   int32_t block;      /* reserved, must be 0 (round 1 offered an L2-blocked Gram-Schmidt here: measured 2x slower than the
-                         streaming kernels on B200 and removed) */
+                         streaming kernels and removed) */
   double atol;
   double rtol;
 } b200_gmres_opts;

@@ -344,7 +344,7 @@ end
 """
     brusselator_function(prob) -> NonlinearFunction{true}
 
-`NonlinearFunction{true}(f!; jvp = jvp!, vjp = vjp!)` whose callables run the fused sm_100a kernels (b1).  With it
+`NonlinearFunction{true}(f!; jvp = jvp!, vjp = vjp!)` whose callables run the fused sm_90a kernels (b1).  With it
 `solve(NonlinearProblem(fn, u0::B200Vector, p), NewtonRaphson(linsolve = B200GMRES()))` runs the reference's own driver
 (`step!`, termination, stats) over device arrays, every arithmetic step in libb200newton.
 """

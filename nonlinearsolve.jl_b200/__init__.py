@@ -1,6 +1,6 @@
-"""nonlinearsolve.jl_b200 — B200-native Newton iteration core behind the NonlinearSolve.jl first-order solver API.
+"""nonlinearsolve.jl_b200 — H100-native Newton iteration core behind the NonlinearSolve.jl first-order solver API.
 
-Only what the hot path needs lives here: `csrc/` (hand-written sm_100a CUDA + the C ABI of include/b200newton.h),
+Only what the hot path needs lives here: `csrc/` (hand-written sm_90a CUDA + the C ABI of include/b200newton.h),
 `_abi.py` (ctypes binding) and `api.py` (host-side mirror of the reference interface).  Import through the root shim
 `nonlinearsolve_jl_b200` (the directory name contains a dot, as the task layout asks).
 """

@@ -1,4 +1,4 @@
-// common.cuh — internal declarations shared by the translation units of libb200newton.so (sm_100a only).
+// common.cuh — internal declarations shared by the translation units of libb200newton.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -11,7 +11,7 @@ struct b200_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  int sm_count = 148;
+  int sm_count = 132;
   size_t smem_optin = 0;
   size_t l2_bytes = 0;
   std::string last_error;

@@ -11,8 +11,8 @@
 //   after an inner panel: TRSM + GEMM (K = 32) on the remaining columns of the outer panel
 //   after the outer panel: row interchanges applied to the columns left/right of it, block TRSM for U12, and the
 //       trailing update  A22 -= L21 U12  with K = NBO — the GEMM-shaped 2/3 n^3 flops — on the FP64 tensor cores
-//       (`gemm_sub_w8_kernel`: mma.sync.m8n8k4.f64 = DMMA.8x8x4 in SASS, the native FP64 MMA shape of sm_100a — m16n8k16
-//       compiles to eight of them; tcgen05 has no FP64 kind).  Look-ahead: the next panel's columns are updated first and
+//       (`gemm_sub_w8_kernel`: mma.sync.m8n8k4.f64 = DMMA.8x8x4 in SASS, the native FP64 MMA shape of sm_90a — m16n8k16
+//       compiles to eight of them; wgmma has no FP64 kind).  Look-ahead: the next panel's columns are updated first and
 //       the panel is factored on a second, HIGHEST-PRIORITY stream underneath the rest of the update.
 // Pivot sequence is LAPACK's (first maximum wins), checked bit-exact against the oracle / scipy in the tests.
 #include "common.cuh"
@@ -122,9 +122,9 @@ __device__ __forceinline__ void block_argmax(double& best, int64_t& bidx, double
 // whole panel.  Per column ONE exchange crosses CTAs, and it carries its own synchronisation (the flag-in-word publication of
 // the resident Arnoldi kernel, NCCL-LL style: every 64-bit word = 32 data bits + a 32-bit epoch, 16-byte stores are single
 // transactions): each CTA publishes {its arg-max, the panel row that holds it} — and CTA 0, which always owns row `col`, that
-// row too — then polls the P headers, picks the pivot (LAPACK idamax rule) and reads the winner's row.  Round 2: this replaced
-// two cooperative-groups grid barriers per column (~2 us each at 64-148 CTAs; the panel sat on the critical path of the last
-// third of the factorisation, profiles/r2_lu_timeline.txt).  Launched cooperatively for the co-residency guarantee only.
+// row too — then polls the P headers, picks the pivot (LAPACK idamax rule) and reads the winner's row.  This replaces
+// two cooperative-groups grid barriers per column (the panel sits on the critical path of the last third of the
+// factorisation).  Launched cooperatively for the co-residency guarantee only.
 constexpr int PX_HREPL = 16, PX_RREPL = 4;   // replicas of the headers / rows (pollers of CTA b read replica b mod R: spreads the hot lines)
 constexpr size_t PX_HDR_WORDS = (size_t)2 * PX_HREPL * PS_MAX * 4;
 constexpr size_t PX_ROW_WORDS = (size_t)2 * PX_RREPL * PS_MAX * 2 * NBI * 2;
@@ -305,7 +305,7 @@ __global__ void __launch_bounds__(DT) trsm_kernel(double* __restrict__ A, int64_
 // shared memory through all kbo / 32 block steps (warp-cooperative solve of the 32 x 32 unit-lower diagonal block — lanes are
 // rows, the solved entries travel by shuffle — then the rows below are updated with the solved block read back as 16-byte
 // broadcasts).  Replaces 31 dependent launches per outer step (16 solves of 32 rows + 15 updates), which had become pure launch
-// latency: 0.73 ms per step even when A12 was 3 500 columns wide (profiles/r2_lu_timeline.txt).  FP64 FMA-bound: kbo^2 / 2 per column.
+// latency even when A12 is thousands of columns wide.  FP64 FMA-bound: kbo^2 / 2 per column.
 constexpr int U12_NCB = 16, U12_T = 256;
 __global__ void __launch_bounds__(U12_T, 2) u12_fused_kernel(double* __restrict__ A, int64_t ld, int64_t k0, int kbo, int64_t k1, int64_t rest) {
   extern __shared__ double xs[];                 // [U12_NCB][kbo] column-major tile of A12
@@ -393,9 +393,8 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 // K is streamed in chunks of 8 through a 4-stage cp.async ring: three chunks are always in flight underneath the MMAs of the
 // current one.  CTA = 8 warps (4 x 2), tile 128 (M) x 64 (N), each warp a 32 x 32 sub-tile = 4 x 4 DMMA m8n8k4 accumulator
 // fragments (64 registers): 119 registers per thread -> two CTAs = 16 warps per SM.  The FP64 tensor pipe of this part is fed
-// by warps, not by tile size (measured at n = 32768, whole getrf): 4 warps x (32 x 64) with 2 CTAs/SM (round 1) 1.38 s, the
-// same kernel at 3 CTAs/SM 1.17 s, this layout 1.08 s; a persistent 128 x 128-tile kernel with 16-byte copies and a chunk
-// stream running across tile boundaries — better arithmetic intensity, ONE 8-warp CTA per SM — 1.57 s.
+// by warps, not by tile size: fewer warps per SM (4 warps x (32 x 64) per CTA, or a persistent 128 x 128-tile kernel with ONE
+// 8-warp CTA per SM despite its better arithmetic intensity) factor the matrix more slowly.
 constexpr int G8_T = 256;
 constexpr int GM_SWZ = 16;  // tile columns per rasterisation group
 template <int MINB, int BK, int STAGES>
@@ -405,8 +404,8 @@ __global__ void __launch_bounds__(G8_T, MINB) gemm_sub_w8_kernel(int64_t M, int6
   double(*As)[BK][GM_BM + GM_PAD] = reinterpret_cast<double(*)[BK][GM_BM + GM_PAD]>(gsm);
   double(*Bs)[BK][GM_BN + GM_PAD] = reinterpret_cast<double(*)[BK][GM_BN + GM_PAD]>(gsm + STAGES * BK * (GM_BM + GM_PAD));
   // Tile order: CTAs are dispatched with blockIdx.x fastest; taken literally every tile column (blockIdx.y) streams the whole
-  // A panel (M x K: 132 MB at n = 32768, K = 512 — more than L2 keeps) from DRAM again: 72 GB of DRAM reads for one trailing
-  // update, L2 hit rate 31 % (ncu, profiles/r2_lu_gemm_launches.csv).  Remapped in groups of GM_SWZ tile columns: consecutive CTAs
+  // A panel (M x K: 132 MB at n = 32768, K = 512 — more than the 50 MB L2 keeps) from DRAM again, tens of GB of DRAM reads for
+  // one trailing update.  Remapped in groups of GM_SWZ tile columns: consecutive CTAs
   // share one A tile and cycle through the group's B tiles (4 MB, L2-resident), so A is read once per group.
   int tile_m = blockIdx.x, tile_n = blockIdx.y;
   {
@@ -900,7 +899,7 @@ int32_t b200_getrf(b200_ctx* ctx, int64_t n, double* A, int64_t ld, int64_t* ipi
       {
         // cooperative panel: as many CTAs as keep >= 128 rows each, at most one per SM (all co-resident)
         const int64_t m = n - c0;
-        // (capping the panel at 64 - 112 CTAs to leave SMs to the concurrent trailing update changes nothing: 1.028 - 1.038 s)
+        // (capping the panel below one CTA per SM to leave SMs to the concurrent trailing update does not help)
         int P = (int)std::min<int64_t>(std::min(ctx->sm_count, PS_MAX), std::max<int64_t>(1, (m + 127) / 128));
         int rpc = (int)((m + P - 1) / P);
         P = (int)((m + rpc - 1) / rpc);
@@ -932,7 +931,7 @@ int32_t b200_getrf(b200_ctx* ctx, int64_t n, double* A, int64_t ld, int64_t* ipi
   // outer block (the K of the trailing update): 512 for the big factorisations halves the C read-modify-write traffic
   // (n = 32768: 1.08 s -> 1.02 s; 768 buys nothing more), 256 below
   const int NBO = n >= 16384 ? 512 : NBO_DEFAULT;  // A/B knob for the outer block
-  const bool trace = getenv("B200_LU_TRACE") != nullptr;  // diagnostic: per-outer-step timeline of the main stream on stderr (profiles/r2_lu_timeline.txt)
+  const bool trace = getenv("B200_LU_TRACE") != nullptr;  // diagnostic: per-outer-step timeline of the main stream on stderr
   std::vector<cudaEvent_t> tev;
   auto mark = [&]() { if (trace) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s_main); tev.push_back(e); } };
   B200_TRY(factor_panel(0, (int)std::min<int64_t>(NBO, n)));

@@ -6,7 +6,7 @@
 // what `solve(ensembleprob, NewtonRaphson(linsolve = KrylovJL_GMRES()), EnsembleThreads(); trajectories)` does per
 // trajectory in the reference (test/PolyAlgorithms/core_tests__item6.jl:3-20).
 //
-// B200 design: a 2D N=32 trajectory has n = 2048 unknowns = 16 KB per vector, so a CTA owns a whole trajectory:
+// Design: a 2D N=32 trajectory has n = 2048 unknowns = 16 KB per vector, so a CTA owns a whole trajectory:
 //   * iterate u and the current Krylov direction v_k live in shared memory (stencil neighbourhoods are read from there),
 //     the vector being orthogonalised w, the residual and the GMRES solution live in registers (8 rows per thread);
 //   * the Krylov basis streams through a per-CTA slab in HBM exactly ONCE per Gram-Schmidt pass: because the CTA owns all

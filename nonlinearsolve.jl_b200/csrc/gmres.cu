@@ -4,7 +4,7 @@
 // lib/NonlinearSolveBase/ext/NonlinearSolveBaseLinearSolveExt.jl:26 (LinearSolve.KrylovJL_GMRES -> Krylov.gmres!):
 // Arnoldi + Gram-Schmidt + Givens reflections, stop at ||r|| <= atol + rtol ||r0||, no restart by default.
 //
-// B200 design: the Krylov basis, the Hessenberg/Givens recurrence, the residual estimate and the stopping decision
+// Design: the Krylov basis, the Hessenberg/Givens recurrence, the residual estimate and the stopping decision
 // all live on the device.  An Arnoldi iteration is a fixed sequence of kernels with no host round trip
 // (operator apply -> multi-dot -> update+norm -> givens -> normalise); the host only polls a status word every
 // `check_every` iterations, and kernels enqueued after convergence early-exit on that word.
@@ -447,6 +447,7 @@ struct ResidentParams {
   const double* nzval;
   int64_t NC;       // cells (opkind 1: half of the rows — the row set is split in two contiguous segments the same way)
   int cpc;          // cells per CTA (even)
+  int qs;           // row pairs per thread held by each shared-memory stage (the rest is read from global memory)
   double a, A;
   const double* u;
   const double* const* V;
@@ -467,8 +468,8 @@ constexpr int LL_MAXG = 160;
 // CTA 0: Hessenberg column -> packed R with the stored Givens rotations, new rotation, residual norm, status (same recurrence
 // as givens_kernel).  The recurrence is serial in i, so one thread runs it — but on a shared-memory copy of the column and of the
 // stored rotations that the whole CTA stages first (and writes back afterwards): run straight on global memory every iteration
-// waits for an L2 round trip (the stores to R may alias the rotations, so the loads cannot be hoisted), ~0.3 us x k per step,
-// which was 7 % of the N = 100 solve.  `ws` = the stage buffers, free once the sweep is over (cap doubles).
+// waits for an L2 round trip (the stores to R may alias the rotations, so the loads cannot be hoisted), a fixed cost x k per step.
+// `ws` = the stage buffers, free once the sweep is over (cap doubles).
 constexpr int R3T = 256;  // = R3_THREADS (declared below)
 __device__ __forceinline__ void resident_givens_tail(const ResidentParams& P, double hbis, double inv, double* ws, int cap, int tid) {
   const int k = P.k;
@@ -523,21 +524,25 @@ __device__ __forceinline__ void resident_givens_tail(const ResidentParams& P, do
 }
 
 // =====================================================================================================================
-// Three-stage, lag-1 organisation of the resident Arnoldi step (rows of one SM fit 54 per thread at 256 threads): the two
-// shared-memory stages are joined by a THIRD stage held in registers (48 more doubles per thread, filled by 128-bit global
-// loads that stay in flight for a whole step, + a small cp.async annex), so three basis vectors are on chip and the
+// Three-stage, lag-1 organisation of the resident Arnoldi step (rows of one SM fit 60 per thread at 256 threads): the two
+// shared-memory stages are joined by a THIRD stage held in registers (32 more doubles per thread, filled by 128-bit global
+// loads that stay in flight for a whole step, + a cp.async annex), so three basis vectors are on chip and the
 // exchange of vector t overlaps the dot products of vector t+1:
 //     h_{t+1} = <v_{t+1}, w_t> - h_t <v_{t+1}, v_t>          (w_t: w before the update with v_t)
 // which are the modified Gram-Schmidt coefficients exactly (the cross product restores the missing update); the pair
 // (<v_{t+1}, w_t>, <v_{t+1}, v_t>) is published before h_t is known.  Stage roles rotate with t mod 3 (0, 1: shared memory
 // via TMA bulk copies, 2: registers).  Exchange: replicated pull tables (16 replicas, 32-byte entries {a, c} with the epoch
 // in every 64-bit word), one entry per polling thread; four table buffers rotate.
+// Capacity: at N = 100 on the 132 SMs of an H100 a CTA owns 15 152 rows, and w plus three whole vectors (485 KB) exceed what
+// one SM holds (64K registers + 227 KB of shared memory).  The shared-memory stages therefore keep the first `qs` row pairs of
+// every thread (the prefix of the CTA's rows that fits beside the annex); the pairs q >= qs of those two stages are read from
+// global memory at each of their two uses — one step apart, so the second read mostly hits the 50 MB L2.
 constexpr int R3_THREADS = 256;
 static_assert(R3T == R3_THREADS, "resident_givens_tail strides by the CTA size");
-constexpr int R3_RP = 27;            // row pairs per thread
-constexpr int R3_ROWS = 2 * R3_RP;   // 54 rows per thread -> at most 13824 rows (6912 cells) per CTA
-constexpr int R3_RPR = 24;           // pairs of the third stage held in registers; the last R3_RP - R3_RPR pairs of each thread
-constexpr int R3_VR = 2 * R3_RPR;    //   sit in a small shared-memory annex filled by cp.async (register budget: 255)
+constexpr int R3_RP = 30;            // row pairs per thread
+constexpr int R3_ROWS = 2 * R3_RP;   // 60 rows per thread -> at most 15360 rows (7680 cells) per CTA
+constexpr int R3_RPR = 16;           // pairs of the third stage held in registers; the last R3_RP - R3_RPR pairs of each thread
+constexpr int R3_VR = 2 * R3_RPR;    //   sit in a shared-memory annex filled by cp.async (register budget: 255, no spills)
 constexpr size_t R3_ANNEX_BYTES = (size_t)(R3_RP - R3_RPR) * R3_THREADS * 16;
 constexpr int R3_REPL = 16;
 constexpr size_t R3_BUF_WORDS = (size_t)R3_REPL * LL_MAXG * 4;
@@ -581,19 +586,32 @@ struct R3Ctx {
   double *stage0, *stage1;
   double2* annex;
   int nrow, ncell, total, k, b, G;
+  int qs;  // row pairs per thread held by the shared-memory stages (>= 1)
 };
 
+// The shared-memory stages hold the CTA's rows [0, 2 * R3_THREADS * qs): a prefix of the first species' segment, or all of it
+// and a prefix of the second species' segment.
 __device__ __forceinline__ void r3_issue_smem(const ResidentParams& P, const R3Ctx& cx, uint64_t* mbar, int t, int stage) {
   if (threadIdx.x == 0 && cx.nrow > 0) {
     const double* src = P.V[t % cx.k];
     double* dst = stage ? cx.stage1 : cx.stage0;
-    const unsigned seg_bytes = (unsigned)cx.ncell * 8u;
+    const int srow = min(cx.nrow, 2 * R3_THREADS * cx.qs);
+    const int r0 = min(srow, cx.ncell), r1 = srow - r0;
     const int64_t c0 = (int64_t)cx.b * P.cpc;
-    mbar_expect_tx(&mbar[stage], 2u * seg_bytes);
-    tma_bulk_load(dst, src + c0, seg_bytes, &mbar[stage]);
-    tma_bulk_load(dst + cx.ncell, src + P.NC + c0, seg_bytes, &mbar[stage]);
+    mbar_expect_tx(&mbar[stage], (unsigned)srow * 8u);
+    tma_bulk_load(dst, src + c0, (unsigned)r0 * 8u, &mbar[stage]);
+    if (r1 > 0) tma_bulk_load(dst + cx.ncell, src + P.NC + c0, (unsigned)r1 * 8u, &mbar[stage]);
   }
 }
+// element pair q (offset lr from this thread's first pair) of a shared-memory-role vector: from the stage `sp` when it holds
+// the pair, else from the vector itself in global memory (`gp` = its first element of this thread, lims / hop as in r3_issue_regs)
+#define R3_SMGET(q, lr, sp, gp, o0, o1)                                                                                         \
+  do {                                                                                                                            \
+    double2 z_;                                                                                                                   \
+    if ((q) < cx.qs) z_ = *reinterpret_cast<const double2*>((sp) + (lr));                                                         \
+    else z_ = __ldg(reinterpret_cast<const double2*>((gp) + (lr) + (((lr) >= lims) ? hop : (int64_t)0)));                        \
+    o0 = z_.x; o1 = z_.y;                                                                                                         \
+  } while (0)
 __device__ __forceinline__ void r3_issue_regs(const ResidentParams& P, const R3Ctx& cx, int t, double (&vr)[R3_VR]) {
   // thread-relative form (constant offsets, two per-thread limits) so that nothing per-q stays live across the step
   const double* src = P.V[t % cx.k] + (int64_t)cx.b * P.cpc + 2 * (int)threadIdx.x;
@@ -645,8 +663,7 @@ __device__ __forceinline__ void r3_apply_operator(const ResidentParams& P, const
   // Built-in Brusselator J(u) v, a PAIR of neighbouring cells per step (the pair never straddles a grid row: the cell count per
   // CTA and N are even), 16-byte loads for everything but the two i-neighbours outside the pair.  Cell coordinates come from two
   // multiplications by reciprocals, exact for these ranges ((c + 1/2) / d is never within 2^-21 of an integer, the product's error
-  // is < 2^-40).  Late round 2: this block used an int64 and an int32 division PER ROW — 13 500 instructions per warp executed
-  // once per launch, 3.8 % of the stall samples of a k = 513 launch, ~100 us of every Arnoldi step whatever the basis size.
+  // is < 2^-40) instead of an int64 and an int32 division per row, a fixed cost of every Arnoldi step whatever the basis size.
   const int N2 = N * N, c0i = (int)c0;
   const double invN = 1.0 / (double)N, invN2 = 1.0 / (double)N2;
   const bool d3 = P.dim == 3;
@@ -751,6 +768,10 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
   const double* sn = (NEXT == 0 ? cx.stage0 : cx.stage1) + 2 * tid;   // next vector if it lives in shared memory
   const bool more = t + 1 < cx.total;
   const int i = t % cx.k;
+  const int lims = cx.ncell - 2 * tid;
+  const int64_t hop = P.NC - cx.ncell;
+  const double* vcur = P.V[i] + (int64_t)cx.b * P.cpc + 2 * tid;                  // current vector in global memory
+  const double* vnext = P.V[(t + 1) % cx.k] + (int64_t)cx.b * P.cpc + 2 * tid;     // next vector in global memory
   const unsigned long long* pollbuf = P.slots + (size_t)(t & 3) * R3_BUF_WORDS;
   unsigned long long ea0, ea1;
   r3g_poll_issue(pollbuf, cx.b, cx.G, ea0, ea1);
@@ -765,9 +786,9 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
         if (lr < lim) {
           double x0, x1, y0, y1;
           if (NEXT == 2) { R3_VRGET(q, x0, x1); }
-          else { const double2 x = *reinterpret_cast<const double2*>(sn + lr); x0 = x.x; x1 = x.y; }
+          else { R3_SMGET(q, lr, sn, vnext, x0, x1); }
           if (ROLE == 2) { R3_VRGET(q, y0, y1); }
-          else { const double2 y = *reinterpret_cast<const double2*>(sc + lr); y0 = y.x; y1 = y.y; }
+          else { R3_SMGET(q, lr, sc, vcur, y0, y1); }
           da = fma(x0, w[2 * q], da); da = fma(x1, w[2 * q + 1], da);
           dc = fma(x0, y0, dc); dc = fma(x1, y1, dc);
         }
@@ -781,7 +802,7 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
         if (lr < lim) {
           double x0, x1;
           if (NEXT == 2) { R3_VRGET(q, x0, x1); }
-          else { const double2 x = *reinterpret_cast<const double2*>(sn + lr); x0 = x.x; x1 = x.y; }
+          else { R3_SMGET(q, lr, sn, vnext, x0, x1); }
           da = fma(x0, w[2 * q], da); db = fma(x1, w[2 * q + 1], db);
         }
       }
@@ -815,7 +836,7 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
       if (lr < lim) {
         double y0, y1;
         if (ROLE == 2) { R3_VRGET(q, y0, y1); }
-        else { const double2 y = *reinterpret_cast<const double2*>(sc + lr); y0 = y.x; y1 = y.y; }
+        else { R3_SMGET(q, lr, sc, vcur, y0, y1); }
         w[2 * q] = fma(-h, y0, w[2 * q]);
         w[2 * q + 1] = fma(-h, y1, w[2 * q + 1]);
       }
@@ -828,7 +849,7 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
       if (lr < lim) {
         double y0, y1;
         if (ROLE == 2) { R3_VRGET(q, y0, y1); }
-        else { const double2 y = *reinterpret_cast<const double2*>(sc + lr); y0 = y.x; y1 = y.y; }
+        else { R3_SMGET(q, lr, sc, vcur, y0, y1); }
         const double w0 = fma(-h, y0, w[2 * q]), w1 = fma(-h, y1, w[2 * q + 1]);
         w[2 * q] = w0; w[2 * q + 1] = w1;
         nacc = fma(w0, w0, nacc); nacc = fma(w1, w1, nacc);
@@ -856,11 +877,12 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
   __shared__ R3GShared sh;
   R3Ctx cx;
   const int cpc = P.cpc;
+  const int sw = min(2 * cpc, 2 * R3_THREADS * P.qs);  // doubles per shared-memory stage
   cx.stage0 = rsm;
-  cx.stage1 = rsm + 2 * cpc;
-  cx.annex = reinterpret_cast<double2*>(rsm + 4 * cpc);
+  cx.stage1 = rsm + sw;
+  cx.annex = reinterpret_cast<double2*>(rsm + 2 * sw);
   const int tid = threadIdx.x, b = blockIdx.x, G = P.G;
-  cx.b = b; cx.G = G; cx.k = P.k; cx.total = P.passes * P.k;
+  cx.b = b; cx.G = G; cx.k = P.k; cx.total = P.passes * P.k; cx.qs = P.qs;
   cx.ncell = (int)max((int64_t)0, min((int64_t)cpc, P.NC - (int64_t)b * cpc));
   cx.nrow = 2 * cx.ncell;
   if (tid == 0) {
@@ -883,13 +905,17 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
   if (total > 2) r3_issue_regs(P, cx, 2, vr);
   {
     if (nrow > 0) mbar_wait(&sh.mbar[0], 0u);
+    const int lims = cx.ncell - 2 * tid;
+    const int64_t hop = P.NC - cx.ncell;
+    const double* g0 = P.V[0] + (int64_t)b * cpc + 2 * tid;
     double da = 0.0;
 #pragma unroll
     for (int q = 0; q < R3_RP; ++q) {
       const int lr = 2 * R3_THREADS * q;
       if (lr < lim) {
-        const double2 x = *reinterpret_cast<const double2*>(cx.stage0 + 2 * tid + lr);
-        da = fma(x.x, w[2 * q], da); da = fma(x.y, w[2 * q + 1], da);
+        double x0, x1;
+        R3_SMGET(q, lr, cx.stage0 + 2 * tid, g0, x0, x1);
+        da = fma(x0, w[2 * q], da); da = fma(x1, w[2 * q + 1], da);
       }
     }
     da = warp_sum(da);
@@ -938,7 +964,7 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
   }
   if (b == 0) {
     if (tid == 0) P.gsub[P.k] = (((gcf[0] + gcf[1]) + (gcf[2] + gcf[3])) + gcf[4]) * inv;  // <v_k, v_{k-1}> for every later Arnoldi step
-    resident_givens_tail(P, hbis, inv, rsm, 4 * cpc, tid);
+    resident_givens_tail(P, hbis, inv, rsm, 2 * sw, tid);
   }
 }
 }  // namespace
@@ -1347,9 +1373,10 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
   // convergence still run the preconditioner's kernels, so the status is polled every other step (default 8 otherwise)
   const int check_every = host_op ? 1 : (o.check_every > 0 ? o.check_every : ((gm->Pl || gm->Pr) ? 2 : 8));
   // resident engine: built-in Brusselator operator with the exact JVP (or an assembled sparse Jacobian), even cell count, one
-  // CTA per SM holds its rows: <= 54 rows per thread and two shared-memory stages + the register stage's annex must fit
+  // CTA per SM holds its rows: <= 60 rows per thread; the register stage's annex and at least one row pair per thread of each
+  // shared-memory stage must fit (the stages hold as many pairs as the shared memory left beside the annex takes)
   bool resident = false;
-  int rs_G = 0, rs_cpc = 0, rs_passes = (orth == B200_ORTH_CGS2) ? 2 : 1;
+  int rs_G = 0, rs_cpc = 0, rs_qs = 0, rs_passes = (orth == B200_ORTH_CGS2) ? 2 : 1;
   int64_t rs_NC = 0;
   size_t rs_smem = 0;
   const bool rs_builtin = op->kind == LINOP_PROBLEM && op->jvp_mode == B200_JVP_EXACT && (op->prob->kind == B200_PROB_BRUSS2D || op->prob->kind == B200_PROB_BRUSS3D);
@@ -1365,14 +1392,18 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
     int64_t cpc = (rs_NC + rs_G - 1) / rs_G;
     cpc = (cpc + 1) & ~(int64_t)1;
     rs_cpc = (int)cpc;
-    rs_smem = sizeof(double) * 4 * (size_t)rs_cpc + R3_ANNEX_BYTES;  // two stages of 2 * cpc rows + the annex of the register stage
-    const bool fits = (rs_NC % 2 == 0) && rs_G <= 159 && (2 * cpc <= (int64_t)R3_ROWS * R3_THREADS) && (rs_smem + 2048 <= ctx->smem_optin);
+    const size_t pair_bytes = 2 * sizeof(double) * 2 * R3_THREADS;  // one row pair per thread in both stages
+    const size_t spare = ctx->smem_optin > R3_ANNEX_BYTES + 2048 ? ctx->smem_optin - R3_ANNEX_BYTES - 2048 : 0;
+    rs_qs = (int)std::min<int64_t>(std::min<int64_t>(R3_RP, (2 * cpc + 2 * R3_THREADS - 1) / (2 * R3_THREADS)), (int64_t)(spare / pair_bytes));
+    const int64_t stage_words = std::min<int64_t>(2 * cpc, (int64_t)2 * R3_THREADS * rs_qs);
+    rs_smem = sizeof(double) * 2 * (size_t)stage_words + R3_ANNEX_BYTES;  // two stages + the annex of the register stage
+    const bool fits = (rs_NC % 2 == 0) && rs_G <= 159 && (2 * cpc <= (int64_t)R3_ROWS * R3_THREADS) && rs_qs >= 1;
     const bool wanted = (o.engine == B200_ENGINE_RESIDENT) || (o.engine == B200_ENGINE_AUTO && n >= 200000);
     if (fits && wanted) {
       resident = true;
       CUDA_TRY(ctx, cudaFuncSetAttribute(resident3g_arnoldi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rs_smem));
     } else if (o.engine == B200_ENGINE_RESIDENT) {
-      return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine: problem does not fit (needs an even cell count and at most ~6800 cells per SM)", __FILE__, __LINE__);
+      return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine: problem does not fit (needs an even cell count and at most 7680 cells per SM)", __FILE__, __LINE__);
     }
   } else if (o.engine == B200_ENGINE_RESIDENT) {
     return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine needs a built-in Brusselator operator with the exact JVP or an assembled sparse Jacobian", __FILE__, __LINE__);
@@ -1458,7 +1489,7 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
           RP.dim = op->prob->kind == B200_PROB_BRUSS2D ? 2 : 3;
           RP.N = op->prob->N; RP.a = op->prob->a; RP.A = op->prob->A; RP.u = op->u;
         }
-        RP.k = k; RP.passes = rs_passes; RP.G = rs_G; RP.NC = rs_NC; RP.cpc = rs_cpc;
+        RP.k = k; RP.passes = rs_passes; RP.G = rs_G; RP.NC = rs_NC; RP.cpc = rs_cpc; RP.qs = rs_qs;
         RP.V = (const double* const*)gm->d_Vptrs; RP.vnew = gm->V[k];
         if (gm->ll_epoch > 0xfff00000u) {  // epoch space nearly exhausted: start over with clean slots
           CUDA_TRY(ctx, cudaMemsetAsync(gm->d_slots, 0, sizeof(unsigned long long) * 4 * R3_BUF_WORDS, ctx->stream));

@@ -114,7 +114,7 @@ __global__ void __launch_bounds__(PB_THREADS) bruss2d_kernel(BrussParams P, cons
 
 // ---- 3D: thread per cell, i fastest -> the centre loads/stores of a warp are one contiguous 256-byte segment per
 // species; i+-1 neighbours hit the same lines in L1, j+-1 / k+-1 neighbours are re-reads served by L1/L2 (the whole
-// 32 MB state of the N=100 case sits in the 126 MB L2), so HBM traffic stays at the algorithmic 2/3/4 Bv.
+// 32 MB state of the N=100 case sits in the 50 MB L2), so HBM traffic stays at the algorithmic 2/3/4 Bv.
 template <int MODE>
 __global__ void __launch_bounds__(PB_THREADS) bruss3d_kernel(BrussParams P, const double* __restrict__ u, const double* __restrict__ d,
                                                               const double* __restrict__ forcing, double* __restrict__ du,
@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(PB_THREADS) bruss3d_kernel(BrussParams P, cons
 }
 
 // ---- 3D, bandwidth-critical form (K1 / K2 of SURVEY.md §8a; north_star: shared-memory halo tile, 16-byte accesses along i,
-// fused norm).  At N = 100 a whole kernel moves 32-48 MB — 5-7 us at the HBM peak — so what decides the time is how many
+// fused norm).  At N = 100 a whole kernel moves 32-48 MB — 10-14 us at the H100's HBM peak — so what decides the time is how many
 // bytes are in flight from the first microsecond on, not the arithmetic.  Organisation:
 //   * a plane (i, j) is N^2 contiguous doubles; the unit of work is a PLANE-CHUNK: TS_L = 2 * TS_THREADS consecutive flat plane
 //     positions of one k plane (a thread: two neighbouring cells, one 16-byte access; N even keeps a pair inside one row).
@@ -192,7 +192,7 @@ __global__ void __launch_bounds__(PB_THREADS) bruss3d_kernel(BrussParams P, cons
 //   * the field that enters through its centre value only (u in the JVP / VJP) rides in the same slot; the forcing plane of
 //     the residual is a per-thread constant;
 //   * outputs go straight to global memory as 16-byte stores; ||f||_inf is folded into the residual's epilogue.
-// HBM traffic: (m + 2) / m of the Laplacian field for a march of m planes (m ~ 6.8 at N = 100 on 296 CTAs: +29 % of ONE of
+// HBM traffic: (m + 2) / m of the Laplacian field for a march of m planes (m ~ 7.6 at N = 100 on 264 CTAs: +26 % of ONE of
 // the two or three vectors, served from L2 for the most part since neighbouring CTAs read the same planes at the same time).
 constexpr int TS_THREADS = 256;
 constexpr int TS_L = 2 * TS_THREADS;
@@ -434,8 +434,8 @@ int32_t launch_bruss(b200_problem* p, const double* u, const double* d, double* 
     if constexpr (tiled) if ((N % 2 == 0) && N2 >= TS_L + 2 * N) {
       constexpr bool has_y = (MODE & (M_JVP | M_VJP)) != 0;
       const size_t slot = sizeof(double) * (2 * (size_t)(TS_L + 2 * N) + (has_y ? 2 * TS_L : 0));
-      // two CTAs per SM share the 227 KB.  Measured at N = 100 (ncu, profiles/r2_stencil_explore.txt): 1 CTA x 16 slots, 2 x 8, 2 x 6,
-      // 2 x 4, 3 x 5, 4 x 4 all land within 10.7 - 13.7 us — the depth of the ring is not what bounds a kernel this short
+      // two CTAs per SM share the 227 KB; the depth of the ring is not what bounds a kernel this short (a few microseconds of
+      // traffic at N = 100), so it stays at up to 8 slots
       const int R = (int)std::min<size_t>(TS_MAXR, (size_t)(100 * 1024) / slot);
       const int per_sm = 2;
       const int chunks = (N2 + TS_L - 1) / TS_L;

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on the B200 box): every kernel family through the C ABI against the CPU oracle
+"""GPU parity tests (run with `-m gpu` on an H100): every kernel family through the C ABI against the CPU oracle
 on the same seeded inputs, plus the committed golden fixtures.  Tolerances are stated per test; integer / index work is
 bit-exact.  Floating point: the reference arithmetic is Float64 throughout; differences come only from FMA contraction
 and reduction order, so 1e-12 relative (scaled by the vector's max) is the bar for single kernels, 1e-6 relative on

@@ -1,5 +1,5 @@
 """Stand-alone K1 / K2 timing (residual f(u), JVP J(u)v, VJP) at N = 100 / 80 on operands that do NOT sit in L2: the kernels cycle
-over SETS buffer triples (SETS * 3 * Bv > 126 MB).  Two clocks: the library's per-launch CUDA events (ctx.profile) and the wall
+over SETS buffer triples (SETS * 3 * Bv > 400 MB, far above the 50 MB L2).  Two clocks: the library's per-launch CUDA events (ctx.profile) and the wall
 clock around a back-to-back batch (launch overhead included).   python tools/stencil_bench.py [N ...]
 Algorithmic bytes: residual 2 Bv (+ the N^2 forcing plane), JVP / VJP 3 Bv."""
 import json
@@ -9,7 +9,7 @@ sys.path.insert(0, ".")
 import numpy as np  # noqa: E402
 import nonlinearsolve_jl_b200 as nls  # noqa: E402
 
-PEAK = json.load(open("MEASURED_PEAKS.json")).get("hbm_gbs", 6572.5) if __import__("os").path.exists("MEASURED_PEAKS.json") else 6572.5
+PEAK = json.load(open("MEASURED_PEAKS.json")).get("hbm_gbs", 3350.0) if __import__("os").path.exists("MEASURED_PEAKS.json") else 3350.0
 ctx = nls.Context(0)
 out = {}
 for N in [int(a) for a in sys.argv[1:]] or [100, 80]:
