@@ -182,6 +182,10 @@ __device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, 
                "l"(gsrc), "r"(bytes), "r"((unsigned)__cvta_generic_to_shared(bar))
                : "memory");
 }
+// bulk prefetch of `bytes` (multiple of 16, 16-byte aligned) of global memory into L2; no completion to wait for
+__device__ __forceinline__ void l2_bulk_prefetch(const void* gsrc, unsigned bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
+}
 
 
 constexpr int32_t B200I_ENS_RC_DEFERRED = -7;  // batched ensemble kernel -> host: redo this trajectory through the general driver (never returned to a caller)

@@ -590,7 +590,9 @@ struct R3Ctx {
 };
 
 // The shared-memory stages hold the CTA's rows [0, 2 * R3_THREADS * qs): a prefix of the first species' segment, or all of it
-// and a prefix of the second species' segment.
+// and a prefix of the second species' segment.  The rows past the stage are read from global memory, one dependent round trip
+// per row pair (the register file is full, nothing is hoisted); they are prefetched into L2 here, two steps before the dot
+// sweep that first reads them, so that round trip ends in L2 instead of HBM.
 __device__ __forceinline__ void r3_issue_smem(const ResidentParams& P, const R3Ctx& cx, uint64_t* mbar, int t, int stage) {
   if (threadIdx.x == 0 && cx.nrow > 0) {
     const double* src = P.V[t % cx.k];
@@ -601,6 +603,13 @@ __device__ __forceinline__ void r3_issue_smem(const ResidentParams& P, const R3C
     mbar_expect_tx(&mbar[stage], (unsigned)srow * 8u);
     tma_bulk_load(dst, src + c0, (unsigned)r0 * 8u, &mbar[stage]);
     if (r1 > 0) tma_bulk_load(dst + cx.ncell, src + P.NC + c0, (unsigned)r1 * 8u, &mbar[stage]);
+    // rows [srow, nrow): the rest of the first species' segment, then the second species' rows from max(srow, ncell) on
+    // (even bounds: every range is a multiple of 16 bytes)
+    if (srow < cx.ncell) l2_bulk_prefetch(src + c0 + srow, (unsigned)(cx.ncell - srow) * 8u);
+    if (srow < cx.nrow) {
+      const int a = max(srow, cx.ncell) - cx.ncell;
+      l2_bulk_prefetch(src + P.NC + c0 + a, (unsigned)(cx.ncell - a) * 8u);
+    }
   }
 }
 // element pair q (offset lr from this thread's first pair) of a shared-memory-role vector: from the stage `sp` when it holds
