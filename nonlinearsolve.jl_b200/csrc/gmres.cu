@@ -17,6 +17,7 @@
 #include "common.cuh"
 #include <math.h>
 #include <float.h>
+#include <stdlib.h>
 #include <algorithm>
 
 namespace {
@@ -1404,6 +1405,15 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
     const size_t pair_bytes = 2 * sizeof(double) * 2 * R3_THREADS;  // one row pair per thread in both stages
     const size_t spare = ctx->smem_optin > R3_ANNEX_BYTES + 2048 ? ctx->smem_optin - R3_ANNEX_BYTES - 2048 : 0;
     rs_qs = (int)std::min<int64_t>(std::min<int64_t>(R3_RP, (2 * cpc + 2 * R3_THREADS - 1) / (2 * R3_THREADS)), (int64_t)(spare / pair_bytes));
+    // diagnostic: cap the stages at fewer row pairs per thread, so that rows move to the global-memory tail (same arithmetic)
+    static_assert(R3_RP == 30, "the message below states the range");
+    if (const char* e = getenv("B200_RESIDENT_STAGE_PAIRS")) {
+      char* end = nullptr;
+      const long cap = strtol(e, &end, 10);
+      if (end == e || *end != '\0' || cap < 1 || cap > R3_RP)
+        return ctx->fail(B200_ERR_INVALID, "B200_RESIDENT_STAGE_PAIRS must be an integer in 1..30 (row pairs per thread of the resident engine's shared-memory stages)", __FILE__, __LINE__);
+      rs_qs = std::min(rs_qs, (int)cap);
+    }
     const int64_t stage_words = std::min<int64_t>(2 * cpc, (int64_t)2 * R3_THREADS * rs_qs);
     rs_smem = sizeof(double) * 2 * (size_t)stage_words + R3_ANNEX_BYTES;  // two stages + the annex of the register stage
     const bool fits = (rs_NC % 2 == 0) && rs_G <= 159 && (2 * cpc <= (int64_t)R3_ROWS * R3_THREADS) && rs_qs >= 1;
