@@ -187,6 +187,30 @@ __device__ __forceinline__ void l2_bulk_prefetch(const void* gsrc, unsigned byte
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
 }
 
+// ---- flag-in-word cross-CTA exchange (the idea of NCCL's LL protocol): a 64-bit value travels as two 64-bit words of
+//      {32 data bits | 32-bit epoch << 32}, written by ONE 16-byte store, so a reader that sees the expected epoch in both words
+//      has the value — no fence, no atomic, no separate barrier, one L2 round trip.  The resident Arnoldi kernel (gmres.cu)
+//      publishes with ll_store; the cooperative LU panel (dense.cu) uses all four parts.
+__device__ __forceinline__ void ll_store(unsigned long long* dst, unsigned long long v, unsigned epoch) {
+  const unsigned long long e = (unsigned long long)epoch << 32;
+  asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1, %2};" ::"l"(dst), "l"((v & 0xffffffffull) | e), "l"((v >> 32) | e) : "memory");
+}
+__device__ __forceinline__ ulonglong2 ll_load(const unsigned long long* src) {
+  ulonglong2 p;
+  asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(p.x), "=l"(p.y) : "l"(src) : "memory");
+  return p;
+}
+// reload `p` from `src` until both words carry `epoch`; bounded so that a fault cannot hang the device: after `bound` reloads
+// *fault = 1 and `p` is left as last read
+__device__ __forceinline__ void ll_wait(const unsigned long long* src, ulonglong2& p, unsigned epoch, unsigned bound, int* fault) {
+  unsigned spins = 0;
+  while ((unsigned)(p.x >> 32) != epoch || (unsigned)(p.y >> 32) != epoch) {
+    if (++spins > bound) { *fault = 1; break; }
+    p = ll_load(src);
+  }
+}
+__device__ __forceinline__ unsigned long long ll_value(ulonglong2 p) { return (p.x & 0xffffffffull) | (p.y << 32); }
+
 
 constexpr int32_t B200I_ENS_RC_DEFERRED = -7;  // batched ensemble kernel -> host: redo this trajectory through the general driver (never returned to a caller)
 

@@ -120,8 +120,7 @@ __device__ __forceinline__ void block_argmax(double& best, int64_t& bidx, double
 // ---- cooperative inner panel: the kbi (<= 32) columns [c0, c0+kbi), rows [c0, n), factored by ONE kernel.  Every CTA keeps
 // its contiguous chunk of panel rows in shared memory (column-major, so a thread-per-row sweep is conflict free) for the
 // whole panel.  Per column ONE exchange crosses CTAs, and it carries its own synchronisation (the flag-in-word publication of
-// the resident Arnoldi kernel, NCCL-LL style: every 64-bit word = 32 data bits + a 32-bit epoch, 16-byte stores are single
-// transactions): each CTA publishes {its arg-max, the panel row that holds it} — and CTA 0, which always owns row `col`, that
+// common.cuh, ll_store / ll_load / ll_wait): each CTA publishes {its arg-max, the panel row that holds it} — and CTA 0, which always owns row `col`, that
 // row too — then polls the P headers, picks the pivot (LAPACK idamax rule) and reads the winner's row.  This replaces
 // two cooperative-groups grid barriers per column (the panel sits on the critical path of the last third of the
 // factorisation).  Launched cooperatively for the co-residency guarantee only.
@@ -129,19 +128,10 @@ constexpr int PX_HREPL = 16, PX_RREPL = 4;   // replicas of the headers / rows (
 constexpr size_t PX_HDR_WORDS = (size_t)2 * PX_HREPL * PS_MAX * 4;
 constexpr size_t PX_ROW_WORDS = (size_t)2 * PX_RREPL * PS_MAX * 2 * NBI * 2;
 constexpr size_t PX_WORDS = PX_HDR_WORDS + PX_ROW_WORDS;
-__device__ __forceinline__ void px_store(unsigned long long* dst, unsigned long long v, unsigned epoch) {
-  const unsigned long long e = (unsigned long long)epoch << 32;
-  asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1, %2};" ::"l"(dst), "l"((v & 0xffffffffull) | e), "l"((v >> 32) | e) : "memory");
-}
 __device__ __forceinline__ unsigned long long px_load(const unsigned long long* src, unsigned epoch, int* fault) {
-  unsigned long long w0, w1;
-  unsigned spins = 0;
-  for (;;) {
-    asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(w0), "=l"(w1) : "l"(src) : "memory");
-    if ((unsigned)(w0 >> 32) == epoch && (unsigned)(w1 >> 32) == epoch) break;
-    if (++spins > (1u << 24)) { *fault = 1; break; }  // bounded: a fault must not hang the device
-  }
-  return (w0 & 0xffffffffull) | (w1 << 32);
+  ulonglong2 p = ll_load(src);
+  ll_wait(src, p, epoch, 1u << 24, fault);
+  return ll_value(p);
 }
 __device__ __forceinline__ size_t px_hdr_at(int buf, int rep, int cta) { return (((size_t)buf * PX_HREPL + rep) * PS_MAX + cta) * 4; }
 __device__ __forceinline__ size_t px_row_at(int buf, int rep, int cta, int kind, int c) {
@@ -183,16 +173,16 @@ __global__ void __launch_bounds__(DT) panel_coop_kernel(int64_t n, double* __res
     if (tid < 32) {
       if (tid < kbi) {
         const double cand = (bidx != INT64_MAX) ? pa[tid * rp + (int)(bidx - row0)] : 0.0;
-        for (int rep = 0; rep < PX_RREPL; ++rep) px_store(xw + px_row_at(buf, rep, b, 0, tid), (unsigned long long)__double_as_longlong(cand), epoch);
+        for (int rep = 0; rep < PX_RREPL; ++rep) ll_store(xw + px_row_at(buf, rep, b, 0, tid), (unsigned long long)__double_as_longlong(cand), epoch);
         if (b == 0) {
           const double cr = pa[tid * rp + (int)(col - row0)];
-          for (int rep = 0; rep < PX_RREPL; ++rep) px_store(xw + px_row_at(buf, rep, 0, 1, tid), (unsigned long long)__double_as_longlong(cr), epoch);
+          for (int rep = 0; rep < PX_RREPL; ++rep) ll_store(xw + px_row_at(buf, rep, 0, 1, tid), (unsigned long long)__double_as_longlong(cr), epoch);
         }
       }
       if (tid < PX_HREPL) {
         unsigned long long* h = xw + px_hdr_at(buf, tid, b);
-        px_store(h, (unsigned long long)__double_as_longlong(best), epoch);
-        px_store(h + 2, (unsigned long long)bidx, epoch);
+        ll_store(h, (unsigned long long)__double_as_longlong(best), epoch);
+        ll_store(h + 2, (unsigned long long)bidx, epoch);
       }
     }
     // (c) poll the P headers, global arg-max (identical in every CTA), pivot bookkeeping

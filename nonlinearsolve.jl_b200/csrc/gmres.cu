@@ -58,6 +58,18 @@ __device__ __forceinline__ void sym_givens(double a, double b, double& c, double
   }
 }
 
+constexpr double GM_BREAKDOWN_TOL = 1.8189894035458565e-12;  // eps(Float64)^(3/4), Krylov.jl breakdown tolerance
+
+// status after Arnoldi step k (1-based) of a cycle: 0 = go on, a B200_LS_* code, or -1 = cycle full (restart: the host resets)
+__device__ __forceinline__ int gm_step_status(double rnorm, double hbis, int k, const GmresState* st) {
+  if (!(rnorm == rnorm) || isinf(rnorm) || !(hbis == hbis) || isinf(hbis)) return B200_LS_NONFINITE;
+  if (rnorm <= st->tol) return B200_LS_SOLVED;
+  if (st->iter_base + k >= st->itmax) return B200_LS_MAXITERS;
+  if (hbis <= GM_BREAKDOWN_TOL) return B200_LS_BREAKDOWN;
+  if (k >= st->kmax_cycle) return -1;
+  return 0;
+}
+
 __device__ __forceinline__ void block_rows(int64_t n, int64_t& r0, int64_t& r1) {
   // contiguous, even-aligned row range of this CTA
   int64_t chunk = (n + gridDim.x - 1) / gridDim.x;
@@ -301,14 +313,7 @@ __global__ void __launch_bounds__(GM_THREADS) givens_kernel(GmresState* __restri
     st->hbis = hbis;
     st->k = k;
     st->inv_h = (hbis > 0.0) ? 1.0 / hbis : 0.0;
-    const double btol = 1.8189894035458565e-12;  // eps(Float64)^(3/4), Krylov.jl breakdown tolerance
-    int status = 0;
-    if (!(rnorm == rnorm) || isinf(rnorm) || !(hbis == hbis) || isinf(hbis)) status = B200_LS_NONFINITE;
-    else if (rnorm <= st->tol) status = B200_LS_SOLVED;
-    else if (st->iter_base + k >= st->itmax) status = B200_LS_MAXITERS;
-    else if (hbis <= btol) status = B200_LS_BREAKDOWN;
-    else if (k >= st->kmax_cycle) status = -1;  // cycle full: restart (host resets)
-    st->status = status;
+    st->status = gm_step_status(rnorm, hbis, k, st);
   }
 }
 
@@ -462,16 +467,17 @@ struct ResidentParams {
   GmresState* st;
 };
 
-// Cross-CTA exchange with the synchronisation folded into the data (the idea of NCCL's LL protocol): each 64-bit word
-// carries 32 data bits and a 32-bit epoch, and 64-bit stores are single transactions, so a reader that sees the expected
-// epoch in every word of an entry has the value — no fence, no atomic, no separate barrier, one L2 round trip.
-constexpr int LL_MAXG = 160;
+// Cross-CTA exchange: flag-in-word tables (common.cuh), one entry per CTA, published with ll_store.  The polls below keep their
+// own loops: rewritten on ll_load / ll_wait they changed the kernel's code and measured slower.
+constexpr int LL_MAXG = 160;                     // CTAs an exchange table has room for
+constexpr int R3_POLLERS = LL_MAXG;              // threads 0 .. R3_POLLERS-1 poll one table entry each (5 warps)
+constexpr int R3_SPARE_POLLER = R3_POLLERS - 1;  // fetches the Gram sub-diagonal entry instead: at most R3_SPARE_POLLER CTAs
+constexpr int R3_THREADS = 256;
 // CTA 0: Hessenberg column -> packed R with the stored Givens rotations, new rotation, residual norm, status (same recurrence
 // as givens_kernel).  The recurrence is serial in i, so one thread runs it — but on a shared-memory copy of the column and of the
 // stored rotations that the whole CTA stages first (and writes back afterwards): run straight on global memory every iteration
 // waits for an L2 round trip (the stores to R may alias the rotations, so the loads cannot be hoisted), a fixed cost x k per step.
 // `ws` = the stage buffers, free once the sweep is over (cap doubles).
-constexpr int R3T = 256;  // = R3_THREADS (declared below)
 __device__ __forceinline__ void resident_givens_tail(const ResidentParams& P, double hbis, double inv, double* ws, int cap, int tid) {
   const int k = P.k;
   GmresState* st = P.st;
@@ -481,7 +487,7 @@ __device__ __forceinline__ void resident_givens_tail(const ResidentParams& P, do
   double *col, *cs, *sn;
   if (staged) {
     col = ws; cs = ws + k; sn = ws + 2 * k;
-    for (int i = tid; i < k; i += R3T) {
+    for (int i = tid; i < k; i += R3_THREADS) {
       const double h = P.h[i];
       col[i] = h; cs[i] = P.cs[i]; sn[i] = P.sn[i];
       if (hr) hr[i] = h;
@@ -509,18 +515,11 @@ __device__ __forceinline__ void resident_givens_tail(const ResidentParams& P, do
     P.z[k] = zeta;
     const double rnorm = fabs(zeta);
     st->rnorm = rnorm; st->hbis = hbis; st->k = k; st->inv_h = inv;
-    int status = 0;
-    if (*P.err) status = B200_LS_NONFINITE;
-    else if (!(rnorm == rnorm) || isinf(rnorm) || !(hbis == hbis) || isinf(hbis)) status = B200_LS_NONFINITE;
-    else if (rnorm <= st->tol) status = B200_LS_SOLVED;
-    else if (st->iter_base + k >= st->itmax) status = B200_LS_MAXITERS;
-    else if (hbis <= 1.8189894035458565e-12) status = B200_LS_BREAKDOWN;
-    else if (k >= st->kmax_cycle) status = -1;
-    st->status = status;
+    st->status = *P.err ? B200_LS_NONFINITE : gm_step_status(rnorm, hbis, k, st);  // an exchange timed out: report, stop
   }
   if (staged) {
     __syncthreads();
-    for (int i = tid; i < k; i += R3T) Rk[i] = col[i];
+    for (int i = tid; i < k; i += R3_THREADS) Rk[i] = col[i];
   }
 }
 
@@ -538,8 +537,6 @@ __device__ __forceinline__ void resident_givens_tail(const ResidentParams& P, do
 // one SM holds (64K registers + 227 KB of shared memory).  The shared-memory stages therefore keep the first `qs` row pairs of
 // every thread (the prefix of the CTA's rows that fits beside the annex); the pairs q >= qs of those two stages are read from
 // global memory at each of their two uses — one step apart, so the second read mostly hits the 50 MB L2.
-constexpr int R3_THREADS = 256;
-static_assert(R3T == R3_THREADS, "resident_givens_tail strides by the CTA size");
 constexpr int R3_RP = 30;            // row pairs per thread
 constexpr int R3_ROWS = 2 * R3_RP;   // 60 rows per thread -> at most 15360 rows (7680 cells) per CTA
 constexpr int R3_RPR = 16;           // pairs of the third stage held in registers; the last R3_RP - R3_RPR pairs of each thread
@@ -548,20 +545,21 @@ constexpr size_t R3_ANNEX_BYTES = (size_t)(R3_RP - R3_RPR) * R3_THREADS * 16;
 constexpr int R3_REPL = 16;
 constexpr size_t R3_BUF_WORDS = (size_t)R3_REPL * LL_MAXG * 4;
 
+constexpr unsigned R3_SPIN_BOUND = 1u << 22;  // exchange polls give up (and flag P.err) after this many reloads
+
+// warp 0: CTA b's entry {a, c} of exchange table `buf`, in every replica
 __device__ __forceinline__ void r3_post(unsigned long long* buf, int b, double a, double c, unsigned epoch) {
-  const int lane = threadIdx.x;  // warp 0 only
+  const int lane = threadIdx.x;
   if (lane < R3_REPL) {
-    const unsigned long long ba = (unsigned long long)__double_as_longlong(a), bc = (unsigned long long)__double_as_longlong(c);
-    const unsigned long long e = (unsigned long long)epoch << 32;
     unsigned long long* dst = buf + ((size_t)lane * LL_MAXG + b) * 4;
-    asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1, %2};" ::"l"(dst), "l"((ba & 0xffffffffull) | e), "l"((ba >> 32) | e) : "memory");
-    asm volatile("st.relaxed.gpu.global.v2.u64 [%0], {%1, %2};" ::"l"(dst + 2), "l"((bc & 0xffffffffull) | e), "l"((bc >> 32) | e) : "memory");
+    ll_store(dst, (unsigned long long)__double_as_longlong(a), epoch);
+    ll_store(dst + 2, (unsigned long long)__double_as_longlong(c), epoch);
   }
 }
-// threads 0..159 poll one entry each; per-warp partial sums land in gA / gC (5 each); caller synchronises
+// threads 0 .. R3_POLLERS-1 poll one entry each, both pairs in flight together; per-warp partial sums land in gA / gC (5 each); caller synchronises
 __device__ __forceinline__ void r3_poll(const unsigned long long* buf, int b, int G, unsigned epoch, int* err, double* gA, double* gC) {
   const int tid = threadIdx.x;
-  if (tid < 160) {
+  if (tid < R3_POLLERS) {
     double xa = 0.0, xc = 0.0;
     if (tid < G) {
       const unsigned long long* src = buf + ((size_t)(b & (R3_REPL - 1)) * LL_MAXG + tid) * 4;
@@ -572,7 +570,7 @@ __device__ __forceinline__ void r3_poll(const unsigned long long* buf, int b, in
         asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(a0), "=l"(a1) : "l"(src) : "memory");
         asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(c0), "=l"(c1) : "l"(src + 2) : "memory");
         ok = ((unsigned)(a0 >> 32) == epoch) && ((unsigned)(a1 >> 32) == epoch) && ((unsigned)(c0 >> 32) == epoch) && ((unsigned)(c1 >> 32) == epoch);
-        if (++spins > (1u << 22)) { *err = 1; break; }
+        if (++spins > R3_SPIN_BOUND) { *err = 1; break; }
       } while (!ok);
       xa = __longlong_as_double((long long)((a0 & 0xffffffffull) | (a1 << 32)));
       xc = __longlong_as_double((long long)((c0 & 0xffffffffull) | (c1 << 32)));
@@ -732,14 +730,14 @@ __device__ __forceinline__ void r3g_poll_issue(const unsigned long long* buf, in
 __device__ __forceinline__ void r3g_poll_finish(const unsigned long long* buf, int b, int G, unsigned epoch, int* err, bool need_c, unsigned long long a0,
                                                 unsigned long long a1, double* gA, double* gC) {
   const int tid = threadIdx.x;
-  if (tid < 160) {
+  if (tid < R3_POLLERS) {
     double xa = 0.0, xc = 0.0;
     if (tid < G) {
       const unsigned long long* src = buf + ((size_t)(b & (R3_REPL - 1)) * LL_MAXG + tid) * 4;
       unsigned spins = 0;
       while (((unsigned)(a0 >> 32) != epoch) || ((unsigned)(a1 >> 32) != epoch)) {
         asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(a0), "=l"(a1) : "l"(src) : "memory");
-        if (++spins > (1u << 22)) { *err = 1; break; }
+        if (++spins > R3_SPIN_BOUND) { *err = 1; break; }
       }
       xa = __longlong_as_double((long long)((a0 & 0xffffffffull) | (a1 << 32)));
       if (need_c) {  // wrap-around step only: the cross product travels in the second pair (same store burst as the first)
@@ -747,7 +745,7 @@ __device__ __forceinline__ void r3g_poll_finish(const unsigned long long* buf, i
         spins = 0;
         do {
           asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(c0), "=l"(c1) : "l"(src + 2) : "memory");
-          if (++spins > (1u << 22)) { *err = 1; break; }
+          if (++spins > R3_SPIN_BOUND) { *err = 1; break; }
         } while (((unsigned)(c0 >> 32) != epoch) || ((unsigned)(c1 >> 32) != epoch));
         xc = __longlong_as_double((long long)((c0 & 0xffffffffull) | (c1 << 32)));
       }
@@ -767,6 +765,10 @@ struct R3GShared {
   double gA[2][8], gC[2][8];      // per-warp sums of the polled exchange entries, by step parity; gC[.][5] = stored cross product
   double hprev[2];                // previous Gram-Schmidt coefficient, by step parity (kept out of the register file)
 };
+static_assert(R3_THREADS == 8 * 32 && R3_POLLERS == 5 * 32, "sum8 / sum5 add the per-warp partials of the CTA / of the polling warps");
+// the fixed summation orders of the per-warp partials (every CTA adds the same numbers in the same order)
+__device__ __forceinline__ double sum8(const double* r) { return ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7])); }
+__device__ __forceinline__ double sum5(const double* g) { return ((g[0] + g[1]) + (g[2] + g[3])) + g[4]; }
 
 template <int ROLE>
 __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3GShared& sh, int t, double (&w)[R3_ROWS], double (&vr)[R3_VR]) {
@@ -821,23 +823,17 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
     da = warp_sum(da);
     if ((tid & 31) == 0) { sh.redA[par][tid >> 5] = da; sh.redC[par][tid >> 5] = dc; }
   }
-  // Gram sub-diagonal entry <v_i, v_{i-1}>, stored when v_i was created: fetched by a spare polling thread (G <= 159)
-  if (tid == 159) sh.gC[par][5] = (i > 0) ? __ldg(P.gsub + i) : 0.0;
+  // Gram sub-diagonal entry <v_i, v_{i-1}>, stored when v_i was created: fetched by the spare polling thread
+  if (tid == R3_SPARE_POLLER) sh.gC[par][R3_POLLERS / 32] = (i > 0) ? __ldg(P.gsub + i) : 0.0;
   r3g_poll_finish(pollbuf, cx.b, cx.G, P.epoch_base + (unsigned)t + 1u, P.err, i == 0 && t > 0, ea0, ea1, sh.gA[par], sh.gC[par]);
   __syncthreads();  // the only barrier of a register-role step
   if (more && tid < 32) {  // warp 0: total of the eight warp partials in a fixed order, then publish for step t+1
-    const double* ra = sh.redA[par];
-    const double* rc = sh.redC[par];
-    const double ta = ((ra[0] + ra[1]) + (ra[2] + ra[3])) + ((ra[4] + ra[5]) + (ra[6] + ra[7]));
-    const double tc = ((rc[0] + rc[1]) + (rc[2] + rc[3])) + ((rc[4] + rc[5]) + (rc[6] + rc[7]));
-    r3_post(P.slots + (size_t)((t + 1) & 3) * R3_BUF_WORDS, cx.b, ta, tc, P.epoch_base + (unsigned)(t + 1) + 1u);
+    r3_post(P.slots + (size_t)((t + 1) & 3) * R3_BUF_WORDS, cx.b, sum8(sh.redA[par]), sum8(sh.redC[par]), P.epoch_base + (unsigned)(t + 1) + 1u);
   }
-  const double* ga = sh.gA[par];
   const double* gc = sh.gC[par];
-  const double sa = ((ga[0] + ga[1]) + (ga[2] + ga[3])) + ga[4];
   // i == 0: first vector of a pass (t == 0: nothing precedes it; t > 0: wrap-around, cross product taken in the sweep of step t-1)
-  const double cross = (i > 0) ? gc[5] : (t > 0 ? (((gc[0] + gc[1]) + (gc[2] + gc[3])) + gc[4]) : 0.0);
-  const double h = sa - sh.hprev[par ^ 1] * cross;
+  const double cross = (i > 0) ? gc[R3_POLLERS / 32] : (t > 0 ? sum5(gc) : 0.0);
+  const double h = sum5(sh.gA[par]) - sh.hprev[par ^ 1] * cross;
   if (tid == 0) sh.hprev[par] = h;
   if (more) {
 #pragma unroll
@@ -932,11 +928,7 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
     if ((tid & 31) == 0) sh.redA[1][tid >> 5] = da;  // parity of "step -1"
     if (tid == 0) sh.hprev[1] = 0.0;
     __syncthreads();
-    if (tid < 32) {
-      const double* ra = sh.redA[1];
-      const double ta = ((ra[0] + ra[1]) + (ra[2] + ra[3])) + ((ra[4] + ra[5]) + (ra[6] + ra[7]));
-      r3_post(P.slots, b, ta, 0.0, P.epoch_base + 1u);
-    }
+    if (tid < 32) r3_post(P.slots, b, sum8(sh.redA[1]), 0.0, P.epoch_base + 1u);
   }
   for (int t = 0; t < total; t += 3) {
     r3g_step<0>(P, cx, sh, t, w, vr);
@@ -947,18 +939,10 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
   //         `total`), Givens (CTA 0), normalise, store v_{k+1}
   const int par = total & 1;
   __syncthreads();
-  if (tid < 32) {
-    const double* ra = sh.redA[par];
-    const double* rc = sh.redC[par];
-    const double ta = ((ra[0] + ra[1]) + (ra[2] + ra[3])) + ((ra[4] + ra[5]) + (ra[6] + ra[7]));
-    const double tc = ((rc[0] + rc[1]) + (rc[2] + rc[3])) + ((rc[4] + rc[5]) + (rc[6] + rc[7]));
-    r3_post(P.slots + (size_t)(total & 3) * R3_BUF_WORDS, b, ta, tc, P.epoch_base + (unsigned)total + 1u);
-  }
+  if (tid < 32) r3_post(P.slots + (size_t)(total & 3) * R3_BUF_WORDS, b, sum8(sh.redA[par]), sum8(sh.redC[par]), P.epoch_base + (unsigned)total + 1u);
   r3_poll(P.slots + (size_t)(total & 3) * R3_BUF_WORDS, b, G, P.epoch_base + (unsigned)total + 1u, P.err, sh.gA[par], sh.gC[par]);
   __syncthreads();
-  const double* gaf = sh.gA[par];
-  const double* gcf = sh.gC[par];
-  const double hbis = sqrt(((gaf[0] + gaf[1]) + (gaf[2] + gaf[3])) + gaf[4]);
+  const double hbis = sqrt(sum5(sh.gA[par]));
   const double inv = hbis > 0.0 ? 1.0 / hbis : 0.0;
   const int ncell = cx.ncell;
   const int64_t NC = P.NC, c0 = (int64_t)b * cpc;
@@ -973,7 +957,7 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
     }
   }
   if (b == 0) {
-    if (tid == 0) P.gsub[P.k] = (((gcf[0] + gcf[1]) + (gcf[2] + gcf[3])) + gcf[4]) * inv;  // <v_k, v_{k-1}> for every later Arnoldi step
+    if (tid == 0) P.gsub[P.k] = sum5(sh.gC[par]) * inv;  // <v_k, v_{k-1}> for every later Arnoldi step
     resident_givens_tail(P, hbis, inv, rsm, 2 * sw, tid);
   }
 }
@@ -995,7 +979,7 @@ struct b200_gmres {
   int64_t hraw_cap;
   GmresState* d_state;
   GmresState* h_state;  // pinned
-  unsigned* d_bar;      // resident engine: error flag (+ legacy barrier counter)
+  int* d_err;           // resident engine: exchange-timeout flag
   unsigned long long* d_slots;  // resident engine: four rotating exchange tables (R3_BUF_WORDS each)
   unsigned ll_epoch;
   b200_linop *Pl, *Pr;   // borrowed preconditioners (apply the inverse)
@@ -1145,6 +1129,107 @@ static int32_t linop_apply_unshifted(b200_linop* op, const double* x, double* y)
   return ctx->fail(B200_ERR_INVALID, "unknown linop kind", __FILE__, __LINE__);
 }
 
+// ------------------------------------------------------------------ resident engine (host side)
+namespace {
+struct ResidentPlan {
+  ResidentParams base;  // the step-independent fields: operator, geometry, passes
+  size_t smem;          // dynamic shared memory of resident3g_arnoldi_kernel: two stages + the annex of the register stage
+};
+
+// raw Hessenberg column k of a capture (b200_gmres_keep_hessenberg), or null when there is none or it is full
+double* gm_hraw(const b200_gmres* gm, int k) { return (gm->d_hraw && (int64_t)k * (k + 3) / 2 <= gm->hraw_cap) ? gm->d_hraw : nullptr; }
+
+// algorithmic bytes of resident Arnoldi step k: the basis once per pass + u, v_k reads + v_{k+1} store
+double resident_step_bytes(int passes, int k, double Bv) { return (passes * (double)k + 3.0) * Bv; }
+
+// Decides whether this solve runs on the resident engine (*use) and, if so, its plan.  Built-in Brusselator operator with the
+// exact JVP (or an assembled sparse Jacobian), even cell count, one CTA per SM holds its rows: <= 60 rows per thread; the
+// register stage's annex and at least one row pair per thread of each shared-memory stage must fit (the stages hold as many
+// pairs as the shared memory left beside the annex takes).  engine = resident fails when any of that does not hold.
+// tests/test_gpu_resident_geometry.py restates this selection independently (its `Geometry` class).
+int32_t gm_resident_plan(b200_gmres* gm, b200_linop* op, bool* use, ResidentPlan* plan) {
+  b200_ctx* ctx = gm->ctx;
+  const b200_gmres_opts& o = gm->opts;
+  const int64_t n = gm->n;
+  *use = false;
+  memset(plan, 0, sizeof(*plan));
+  const bool builtin = op->kind == LINOP_PROBLEM && op->jvp_mode == B200_JVP_EXACT && (op->prob->kind == B200_PROB_BRUSS2D || op->prob->kind == B200_PROB_BRUSS3D);
+  const bool csr = op->kind == LINOP_SPARSE_JAC && n % 2 == 0;
+  const bool precond = gm->Pl || gm->Pr;
+  if (precond && o.engine == B200_ENGINE_RESIDENT)
+    return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine does not take preconditioners (use engine = auto / multikernel)", __FILE__, __LINE__);
+  if (op->shift != 0.0 && o.engine == B200_ENGINE_RESIDENT)
+    return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine does not take shifted operators (use engine = auto / multikernel)", __FILE__, __LINE__);
+  if (o.engine == B200_ENGINE_MULTIKERNEL || !(builtin || csr) || precond || op->shift != 0.0) {
+    if (o.engine == B200_ENGINE_RESIDENT)
+      return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine needs a built-in Brusselator operator with the exact JVP or an assembled sparse Jacobian", __FILE__, __LINE__);
+    return B200_OK;
+  }
+  ResidentParams& RP = plan->base;
+  RP.passes = (o.orth == B200_ORTH_CGS2) ? 2 : 1;
+  RP.NC = n / 2;
+  RP.G = ctx->sm_count;
+  int64_t cpc = (RP.NC + RP.G - 1) / RP.G;
+  cpc = (cpc + 1) & ~(int64_t)1;
+  RP.cpc = (int)cpc;
+  const size_t pair_bytes = 2 * sizeof(double) * 2 * R3_THREADS;  // one row pair per thread in both stages
+  const size_t spare = ctx->smem_optin > R3_ANNEX_BYTES + 2048 ? ctx->smem_optin - R3_ANNEX_BYTES - 2048 : 0;
+  RP.qs = (int)std::min<int64_t>(std::min<int64_t>(R3_RP, (2 * cpc + 2 * R3_THREADS - 1) / (2 * R3_THREADS)), (int64_t)(spare / pair_bytes));
+  // diagnostic: cap the stages at fewer row pairs per thread, so that rows move to the global-memory tail (same arithmetic)
+  static_assert(R3_RP == 30, "the message below states the range");
+  if (const char* e = getenv("B200_RESIDENT_STAGE_PAIRS")) {
+    char* end = nullptr;
+    const long cap = strtol(e, &end, 10);
+    if (end == e || *end != '\0' || cap < 1 || cap > R3_RP)
+      return ctx->fail(B200_ERR_INVALID, "B200_RESIDENT_STAGE_PAIRS must be an integer in 1..30 (row pairs per thread of the resident engine's shared-memory stages)", __FILE__, __LINE__);
+    RP.qs = std::min(RP.qs, (int)cap);
+  }
+  const int64_t stage_words = std::min<int64_t>(2 * cpc, (int64_t)2 * R3_THREADS * RP.qs);
+  plan->smem = sizeof(double) * 2 * (size_t)stage_words + R3_ANNEX_BYTES;
+  const bool fits = (RP.NC % 2 == 0) && RP.G <= R3_SPARE_POLLER && (2 * cpc <= (int64_t)R3_ROWS * R3_THREADS) && RP.qs >= 1;
+  const bool wanted = (o.engine == B200_ENGINE_RESIDENT) || (o.engine == B200_ENGINE_AUTO && n >= 200000);
+  if (!fits || !wanted) {
+    if (o.engine == B200_ENGINE_RESIDENT)
+      return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine: problem does not fit (needs an even cell count and at most 7680 cells per SM)", __FILE__, __LINE__);
+    return B200_OK;
+  }
+  if (csr) {
+    RP.opkind = 1;
+    b200i_sparse_jac_csr(op->sj, &RP.rowptr, &RP.csr_col, &RP.csr_map);
+    RP.nzval = op->nzval;
+  } else {
+    RP.dim = op->prob->kind == B200_PROB_BRUSS2D ? 2 : 3;
+    RP.N = op->prob->N; RP.a = op->prob->a; RP.A = op->prob->A; RP.u = op->u;
+  }
+  CUDA_TRY(ctx, cudaFuncSetAttribute(resident3g_arnoldi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan->smem));
+  *use = true;
+  return B200_OK;
+}
+
+// Arnoldi step k on the resident engine: one cooperative kernel, JVP -> (iterated) MGS with TMA-staged basis -> norm -> Givens -> v_{k+1}
+int32_t gm_resident_step(b200_gmres* gm, const ResidentPlan& plan, int k) {
+  b200_ctx* ctx = gm->ctx;
+  ResidentParams RP = plan.base;
+  RP.k = k;
+  RP.V = (const double* const*)gm->d_Vptrs; RP.vnew = gm->V[k];
+  if (gm->ll_epoch > 0xfff00000u) {  // epoch space nearly exhausted: start over with clean slots
+    CUDA_TRY(ctx, cudaMemsetAsync(gm->d_slots, 0, sizeof(unsigned long long) * 4 * R3_BUF_WORDS, ctx->stream));
+    gm->ll_epoch = 0;
+  }
+  RP.slots = gm->d_slots; RP.epoch_base = gm->ll_epoch; RP.err = gm->d_err;
+  gm->ll_epoch += (unsigned)(RP.passes * k + 2);
+  RP.h = gm->d_h; RP.gsub = gm->d_gsub; RP.R = gm->d_R; RP.cs = gm->d_cs; RP.sn = gm->d_sn; RP.z = gm->d_z;
+  RP.hraw = gm_hraw(gm, k);
+  RP.st = gm->d_state;
+  void* args[] = {&RP};
+  if (ctx->prof_on) ctx->prof_begin(B200_KID_RESIDENT, resident_step_bytes(RP.passes, k, 8.0 * (double)gm->n));
+  CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)resident3g_arnoldi_kernel, dim3(RP.G), dim3(R3_THREADS), args, plan.smem, ctx->stream));
+  ctx->launches++;
+  if (ctx->prof_on) ctx->prof_end();
+  return B200_OK;
+}
+}  // namespace
+
 extern "C" {
 int32_t b200_gemv(b200_ctx* ctx, int32_t trans, int64_t m, int64_t n, const double* A, int64_t ld, const double* x, double* y) {
   B200_DEVICE_GUARD(ctx);
@@ -1263,7 +1348,7 @@ int32_t b200_gmres_create(b200_ctx* ctx, int64_t n, const b200_gmres_opts* opts,
   gm->kcap = 0; gm->d_Vptrs = nullptr; gm->vptr_cap = 0;
   gm->d_h = gm->d_hacc = gm->d_R = gm->d_cs = gm->d_sn = gm->d_z = gm->d_y = gm->d_partial = gm->d_gsub = nullptr;
   gm->d_hraw = nullptr; gm->hraw_cap = 0;
-  gm->d_bar = nullptr; gm->d_slots = nullptr; gm->ll_epoch = 0; gm->Pl = gm->Pr = nullptr; gm->pt1 = gm->pt2 = nullptr;
+  gm->d_err = nullptr; gm->d_slots = nullptr; gm->ll_epoch = 0; gm->Pl = gm->Pr = nullptr; gm->pt1 = gm->pt2 = nullptr;
   // streaming grid: 4 CTAs of 256 threads per SM, fewer for small n (at least 512 rows per CTA)
   int64_t g = std::min<int64_t>((int64_t)ctx->sm_count * 4, std::max<int64_t>(1, n / 512));
   gm->G = (int)g;
@@ -1274,10 +1359,10 @@ int32_t b200_gmres_create(b200_ctx* ctx, int64_t n, const b200_gmres_opts* opts,
   CUDA_TRY(ctx, cudaMalloc(&gm->d_norm_partial2, sizeof(double) * std::max(gm->G, B200_RED_MAX_BLOCKS)));
   CUDA_TRY(ctx, cudaMalloc(&gm->d_state, sizeof(GmresState)));
   CUDA_TRY(ctx, cudaMallocHost(&gm->h_state, sizeof(GmresState)));
-  CUDA_TRY(ctx, cudaMalloc(&gm->d_bar, 4 * sizeof(unsigned)));
+  CUDA_TRY(ctx, cudaMalloc(&gm->d_err, sizeof(int)));
   CUDA_TRY(ctx, cudaMalloc(&gm->d_slots, sizeof(unsigned long long) * 4 * R3_BUF_WORDS));
   CUDA_TRY(ctx, cudaMemsetAsync(gm->d_slots, 0, sizeof(unsigned long long) * 4 * R3_BUF_WORDS, ctx->stream));
-  CUDA_TRY(ctx, cudaMemsetAsync(gm->d_bar, 0, 4 * sizeof(unsigned), ctx->stream));
+  CUDA_TRY(ctx, cudaMemsetAsync(gm->d_err, 0, sizeof(int), ctx->stream));
   CUDA_TRY(ctx, cudaFuncSetAttribute(update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * (GM_KCAP + 64))));
   CUDA_TRY(ctx, cudaFuncSetAttribute(backsolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * (GM_KCAP + 64))));
   int mem = opts->restart > 0 ? opts->restart : (opts->memory > 0 ? opts->memory : 20);
@@ -1297,7 +1382,7 @@ int32_t b200_gmres_destroy(b200_gmres* gm) {
   cudaFree(gm->w); cudaFree(gm->r0); cudaFree(gm->d_norm_partial); cudaFree(gm->d_norm_partial2); cudaFree(gm->d_state);
   if (gm->d_hraw) cudaFree(gm->d_hraw);
   cudaFreeHost(gm->h_state);
-  if (gm->d_bar) cudaFree(gm->d_bar);
+  if (gm->d_err) cudaFree(gm->d_err);
   if (gm->d_slots) cudaFree(gm->d_slots);
   if (gm->pt1) cudaFree(gm->pt1);
   if (gm->pt2) cudaFree(gm->pt2);
@@ -1382,51 +1467,10 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
   // with a preconditioner an iteration is expensive (a V-cycle per step) and the basis short: iterations enqueued after
   // convergence still run the preconditioner's kernels, so the status is polled every other step (default 8 otherwise)
   const int check_every = host_op ? 1 : (o.check_every > 0 ? o.check_every : ((gm->Pl || gm->Pr) ? 2 : 8));
-  // resident engine: built-in Brusselator operator with the exact JVP (or an assembled sparse Jacobian), even cell count, one
-  // CTA per SM holds its rows: <= 60 rows per thread; the register stage's annex and at least one row pair per thread of each
-  // shared-memory stage must fit (the stages hold as many pairs as the shared memory left beside the annex takes)
-  bool resident = false;
-  int rs_G = 0, rs_cpc = 0, rs_qs = 0, rs_passes = (orth == B200_ORTH_CGS2) ? 2 : 1;
-  int64_t rs_NC = 0;
-  size_t rs_smem = 0;
-  const bool rs_builtin = op->kind == LINOP_PROBLEM && op->jvp_mode == B200_JVP_EXACT && (op->prob->kind == B200_PROB_BRUSS2D || op->prob->kind == B200_PROB_BRUSS3D);
-  const bool rs_csr = op->kind == LINOP_SPARSE_JAC && n % 2 == 0;
   b200_linop *Pl = gm->Pl, *Pr = gm->Pr;
-  if ((Pl || Pr) && o.engine == B200_ENGINE_RESIDENT)
-    return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine does not take preconditioners (use engine = auto / multikernel)", __FILE__, __LINE__);
-  if (op->shift != 0.0 && o.engine == B200_ENGINE_RESIDENT)
-    return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine does not take shifted operators (use engine = auto / multikernel)", __FILE__, __LINE__);
-  if (o.engine != B200_ENGINE_MULTIKERNEL && (rs_builtin || rs_csr) && !Pl && !Pr && op->shift == 0.0) {
-    rs_NC = n / 2;
-    rs_G = ctx->sm_count;
-    int64_t cpc = (rs_NC + rs_G - 1) / rs_G;
-    cpc = (cpc + 1) & ~(int64_t)1;
-    rs_cpc = (int)cpc;
-    const size_t pair_bytes = 2 * sizeof(double) * 2 * R3_THREADS;  // one row pair per thread in both stages
-    const size_t spare = ctx->smem_optin > R3_ANNEX_BYTES + 2048 ? ctx->smem_optin - R3_ANNEX_BYTES - 2048 : 0;
-    rs_qs = (int)std::min<int64_t>(std::min<int64_t>(R3_RP, (2 * cpc + 2 * R3_THREADS - 1) / (2 * R3_THREADS)), (int64_t)(spare / pair_bytes));
-    // diagnostic: cap the stages at fewer row pairs per thread, so that rows move to the global-memory tail (same arithmetic)
-    static_assert(R3_RP == 30, "the message below states the range");
-    if (const char* e = getenv("B200_RESIDENT_STAGE_PAIRS")) {
-      char* end = nullptr;
-      const long cap = strtol(e, &end, 10);
-      if (end == e || *end != '\0' || cap < 1 || cap > R3_RP)
-        return ctx->fail(B200_ERR_INVALID, "B200_RESIDENT_STAGE_PAIRS must be an integer in 1..30 (row pairs per thread of the resident engine's shared-memory stages)", __FILE__, __LINE__);
-      rs_qs = std::min(rs_qs, (int)cap);
-    }
-    const int64_t stage_words = std::min<int64_t>(2 * cpc, (int64_t)2 * R3_THREADS * rs_qs);
-    rs_smem = sizeof(double) * 2 * (size_t)stage_words + R3_ANNEX_BYTES;  // two stages + the annex of the register stage
-    const bool fits = (rs_NC % 2 == 0) && rs_G <= 159 && (2 * cpc <= (int64_t)R3_ROWS * R3_THREADS) && rs_qs >= 1;
-    const bool wanted = (o.engine == B200_ENGINE_RESIDENT) || (o.engine == B200_ENGINE_AUTO && n >= 200000);
-    if (fits && wanted) {
-      resident = true;
-      CUDA_TRY(ctx, cudaFuncSetAttribute(resident3g_arnoldi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rs_smem));
-    } else if (o.engine == B200_ENGINE_RESIDENT) {
-      return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine: problem does not fit (needs an even cell count and at most 7680 cells per SM)", __FILE__, __LINE__);
-    }
-  } else if (o.engine == B200_ENGINE_RESIDENT) {
-    return ctx->fail(B200_ERR_UNSUPPORTED, "resident GMRES engine needs a built-in Brusselator operator with the exact JVP or an assembled sparse Jacobian", __FILE__, __LINE__);
-  }
+  bool resident = false;
+  ResidentPlan rs;
+  B200_TRY(gm_resident_plan(gm, op, &resident, &rs));
   const int64_t itmax = o.itmax > 0 ? o.itmax : n;
   const int restart_len = o.restart > 0 ? (int)std::min<int64_t>(o.restart, n) : 0;
   const int ew_grid = (int)std::min<int64_t>((n + GM_THREADS * 2 - 1) / (GM_THREADS * 2), (int64_t)ctx->sm_count * 8);
@@ -1443,7 +1487,7 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
   init.atol = o.atol;
   init.rtol = o.rtol;
   *gm->h_state = init;
-  CUDA_TRY(ctx, cudaMemsetAsync(gm->d_bar, 0, 4 * sizeof(unsigned), ctx->stream));  // resident engine: exchange-timeout flag of a previous solve
+  CUDA_TRY(ctx, cudaMemsetAsync(gm->d_err, 0, sizeof(int), ctx->stream));  // resident engine: exchange-timeout flag of a previous solve
   CUDA_TRY(ctx, cudaMemcpyAsync(gm->d_state, gm->h_state, sizeof(GmresState), cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // h_state is reused as the read-back buffer below
 
@@ -1497,36 +1541,9 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
       if (rc == B200_ERR_NOMEM || k + 40 > GM_KCAP) { oom = 1; --k; break; }
       B200_TRY(rc);
       if (resident) {
-        // one cooperative kernel: JVP -> (iterated) MGS with TMA-staged basis -> norm -> Givens -> v_{k+1}
-        ResidentParams RP;
-        memset(&RP, 0, sizeof(RP));
-        if (rs_csr) {
-          RP.opkind = 1;
-          b200i_sparse_jac_csr(op->sj, &RP.rowptr, &RP.csr_col, &RP.csr_map);
-          RP.nzval = op->nzval;
-        } else {
-          RP.dim = op->prob->kind == B200_PROB_BRUSS2D ? 2 : 3;
-          RP.N = op->prob->N; RP.a = op->prob->a; RP.A = op->prob->A; RP.u = op->u;
-        }
-        RP.k = k; RP.passes = rs_passes; RP.G = rs_G; RP.NC = rs_NC; RP.cpc = rs_cpc; RP.qs = rs_qs;
-        RP.V = (const double* const*)gm->d_Vptrs; RP.vnew = gm->V[k];
-        if (gm->ll_epoch > 0xfff00000u) {  // epoch space nearly exhausted: start over with clean slots
-          CUDA_TRY(ctx, cudaMemsetAsync(gm->d_slots, 0, sizeof(unsigned long long) * 4 * R3_BUF_WORDS, ctx->stream));
-          gm->ll_epoch = 0;
-        }
-        RP.slots = gm->d_slots; RP.epoch_base = gm->ll_epoch; RP.err = reinterpret_cast<int*>(gm->d_bar + 1);
-        gm->ll_epoch += (unsigned)(rs_passes * k + 2);
-        RP.h = gm->d_h; RP.gsub = gm->d_gsub; RP.R = gm->d_R; RP.cs = gm->d_cs; RP.sn = gm->d_sn; RP.z = gm->d_z;
-        RP.hraw = (gm->d_hraw && (int64_t)k * (k + 3) / 2 <= gm->hraw_cap) ? gm->d_hraw : nullptr;
-        RP.st = gm->d_state;
-        void* args[] = {&RP};
-        if (ctx->prof_on) ctx->prof_begin(B200_KID_RESIDENT, (rs_passes * (double)k + 3.0) * Bv);
-        CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)resident3g_arnoldi_kernel, dim3(rs_G), dim3(R3_THREADS), args, rs_smem, ctx->stream));
-        ctx->launches++;
-        if (ctx->prof_on) ctx->prof_end();
+        B200_TRY(gm_resident_step(gm, rs, k));
       } else {
-      // w = M^-1 A N^-1 v_k
-      {
+        // w = M^-1 A N^-1 v_k
         const double* in = gm->V[k - 1];
         if (Pr) { B200_TRY(b200i_linop_apply(Pr, in, gm->pt1)); in = gm->pt1; bytes += 3 * Bv; }
         if (Pl) {
@@ -1536,23 +1553,20 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
         } else {
           B200_TRY(b200i_linop_apply(op, in, gm->w));
         }
-      }
-      if (orth == B200_ORTH_MGS) {
-        double* pin = gm->d_norm_partial;
-        double* pout = gm->d_norm_partial2;
-        PLAUNCH(ctx, B200_KID_MGS, 2.0 * Bv, mgs_pass_kernel, G, GM_THREADS, 0, gm->d_state, (const double*)nullptr, (const double*)gm->V[0], -1, pin, pout, gm->d_h,
-               gm->w, n);
-        for (int i = 0; i < k; ++i) {
-          std::swap(pin, pout);
-          PLAUNCH(ctx, B200_KID_MGS, 4.0 * Bv, mgs_pass_kernel, G, GM_THREADS, 0, gm->d_state, (const double*)gm->V[i],
-                 (const double*)(i + 1 < k ? gm->V[i + 1] : nullptr), i, pin, pout, gm->d_h, gm->w, n);
-        }
-        PLAUNCH(ctx, B200_KID_GIVENS, 0.0, givens_kernel, 1, GM_THREADS, 0, gm->d_state, k, G, pout, gm->d_h, gm->d_R, gm->d_cs, gm->d_sn, gm->d_z,
-               (gm->d_hraw && (int64_t)k * (k + 3) / 2 <= gm->hraw_cap) ? gm->d_hraw : nullptr);
-      } else {
-        const size_t shm = sizeof(double) * (k + 32);
-        const int passes = (orth == B200_ORTH_CGS2) ? 2 : 1;
-        {
+        const double* norm_partial = gm->d_norm_partial;
+        if (orth == B200_ORTH_MGS) {
+          double* pin = gm->d_norm_partial;
+          double* pout = gm->d_norm_partial2;
+          PLAUNCH(ctx, B200_KID_MGS, 2.0 * Bv, mgs_pass_kernel, G, GM_THREADS, 0, gm->d_state, (const double*)nullptr, (const double*)gm->V[0], -1, pin, pout, gm->d_h,
+                  gm->w, n);
+          for (int i = 0; i < k; ++i) {
+            std::swap(pin, pout);
+            PLAUNCH(ctx, B200_KID_MGS, 4.0 * Bv, mgs_pass_kernel, G, GM_THREADS, 0, gm->d_state, (const double*)gm->V[i],
+                    (const double*)(i + 1 < k ? gm->V[i + 1] : nullptr), i, pin, pout, gm->d_h, gm->w, n);
+          }
+          norm_partial = pout;
+        } else {
+          const size_t shm = sizeof(double) * (k + 32);
           PLAUNCH(ctx, B200_KID_MULTIDOT, (k + 1.0) * Bv, multidot_kernel, G, GM_THREADS, 0, gm->d_state, (const double* const*)gm->d_Vptrs, k, gm->w, n, gm->d_partial);
           LAUNCH(ctx, reduce_h_kernel, (k + 7) / 8, GM_THREADS, 0, gm->d_state, k, G, gm->d_partial, gm->d_h, (double*)nullptr);
           PLAUNCH(ctx, B200_KID_UPDATE, (k + 2.0) * Bv, update_kernel, G, GM_THREADS, shm, gm->d_state, 0, (const double* const*)gm->d_Vptrs, k, gm->d_h, -1.0, gm->w, gm->w, n,
@@ -1564,11 +1578,10 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
                     gm->w, n, gm->d_norm_partial);
           }
         }
-        PLAUNCH(ctx, B200_KID_GIVENS, 0.0, givens_kernel, 1, GM_THREADS, 0, gm->d_state, k, G, gm->d_norm_partial, gm->d_h, gm->d_R, gm->d_cs, gm->d_sn, gm->d_z,
-               (gm->d_hraw && (int64_t)k * (k + 3) / 2 <= gm->hraw_cap) ? gm->d_hraw : nullptr);
+        PLAUNCH(ctx, B200_KID_GIVENS, 0.0, givens_kernel, 1, GM_THREADS, 0, gm->d_state, k, G, norm_partial, gm->d_h, gm->d_R, gm->d_cs, gm->d_sn, gm->d_z,
+                gm_hraw(gm, k));
+        PLAUNCH(ctx, B200_KID_NORMALIZE, 2.0 * Bv, normalize_kernel, ew_grid, GM_THREADS, 0, gm->d_state, 1, gm->w, gm->V[k], n);
       }
-      PLAUNCH(ctx, B200_KID_NORMALIZE, 2.0 * Bv, normalize_kernel, ew_grid, GM_THREADS, 0, gm->d_state, 1, gm->w, gm->V[k], n);
-      }  // multi-kernel engine
       CHECK_LAUNCH(ctx);
       const bool must_check = (k % check_every == 0) || (iters_total + k >= itmax) || (restart_len > 0 && k >= restart_len);
       if (must_check) {
@@ -1589,7 +1602,7 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
     //   CGS (2j+2) Bv | CGS2 (4j+4) Bv | MGS (3j+1) Bv (dot pass reads v_{i+1}, update pass reads v_i, w read+written)
     for (int j = 1; j <= k; ++j) {
       double orthb = (orth == B200_ORTH_CGS) ? (2.0 * j + 2.0) : (orth == B200_ORTH_CGS2) ? (4.0 * j + 4.0) : (3.0 * j + 1.0);
-      if (resident) bytes += (rs_passes * (double)j + 3.0) * Bv;  // basis once per pass + u, v_k reads + v_{k+1} store
+      if (resident) bytes += resident_step_bytes(rs.base.passes, j, Bv);
       else bytes += (3.0 + 2.0 + orthb) * Bv;
     }
     // x += V_k y
@@ -1625,8 +1638,8 @@ int32_t b200_gmres_solve(b200_gmres* gm, b200_linop* op, const double* b, double
   }
   B200_TRY(gm_fetch_state(gm));
   if (resident && final_status == B200_LS_NONFINITE) {  // tell an exchange time-out (bounded spin) from a numerical NaN / Inf
-    unsigned flag = 0;
-    CUDA_TRY(ctx, cudaMemcpy(&flag, gm->d_bar + 1, sizeof(unsigned), cudaMemcpyDeviceToHost));
+    int flag = 0;
+    CUDA_TRY(ctx, cudaMemcpy(&flag, gm->d_err, sizeof(int), cudaMemcpyDeviceToHost));
     if (flag) ctx->fail(B200_OK, "resident GMRES engine: a cross-CTA exchange timed out (bounded spin); the solve is reported as B200_LS_NONFINITE", __FILE__, __LINE__);
   }
   st_local.status = final_status;
