@@ -14,7 +14,9 @@
 //       (`gemm_sub_w8_kernel`: mma.sync.m8n8k4.f64 = DMMA.8x8x4 in SASS, the native FP64 MMA shape of sm_90a — m16n8k16
 //       compiles to eight of them; wgmma has no FP64 kind).  Look-ahead: the next panel's columns are updated first and
 //       the panel is factored on a second, HIGHEST-PRIORITY stream underneath the rest of the update.
-// Pivot sequence is LAPACK's (first maximum wins), checked bit-exact against the oracle / scipy in the tests.
+// Pivot rule is LAPACK's (largest magnitude, first index wins ties).  tests/test_gpu_dense_lu.py checks the factorisation in
+// every blocking regime up to n = 32768: LAPACK's pivots up to its first ambiguous column and on exactly constructed ties,
+// |L| <= 1, Higham's componentwise error bounds for getrf and getrs, info on exactly zero columns, and bit-identical repeats.
 #include "common.cuh"
 #include <math.h>
 #include <algorithm>
