@@ -1114,12 +1114,13 @@ def shard_range(K, rank, world_size):
 
 
 class EnsembleCache:
-    """Persistent per-GPU batch workspace for K_local 2D-Brusselator trajectories."""
+    """Persistent per-GPU batch workspace for K_local 2D-Brusselator trajectories.  The options are those of a single solve;
+    option sets the batched kernel does not implement (see csrc/ens_batched.cu) run each trajectory through the general driver."""
 
-    def __init__(self, ctx, N, nprob_local, alpha, alg, abstol=None, reltol=None, maxiters=1000):
+    def __init__(self, ctx, N, nprob_local, alpha, alg, abstol=None, reltol=None, maxiters=1000, termination_condition=None, maxtime=None):
         self.ctx, self.N, self.K, self.n = ctx, N, nprob_local, 2 * N * N
         dummy = NonlinearProblem(Brusselator2D(N), None, (3.4, 1.0, alpha))
-        self.opts = _build_opts(dummy, alg, abstol, reltol, maxiters, None, False)
+        self.opts = _build_opts(dummy, alg, abstol, reltol, maxiters, termination_condition, False, maxtime)
         self._h = C.c_void_p()
         check(ctx.handle, lib().b200_ens_create(ctx.handle, N, nprob_local, float(alpha), C.byref(self.opts), C.byref(self._h)))
         self._fin = ctx._adopt(weakref.finalize(self, lib().b200_ens_destroy, self._h))

@@ -6,6 +6,12 @@
 // what `solve(ensembleprob, NewtonRaphson(linsolve = KrylovJL_GMRES()), EnsembleThreads(); trajectories)` does per
 // trajectory in the reference (test/PolyAlgorithms/core_tests__item6.jl:3-20).
 //
+// Option sets batched here (b200i_ens_batched_supported): exact JVP; unrestarted GMRES with MGS or CGS2 (MGS applied twice),
+// any itmax / atol / rtol, optional EW forcing; termination AbsNorm, AbsNormSafe or AbsNormSafeBest on the inf-norm with the
+// default step-stall window (32); no maxtime; N <= 32.  Every other option set (the Norm / Rel / Abs modes, the L2 norm,
+// another stall window, one-pass CGS, a wall-clock limit, FD-JVP, warm start, restart, N > 32) runs each trajectory
+// through the general driver of newton.cu instead (b200_ens_solve).  tests/test_gpu_ensemble.py checks both routes.
+//
 // Design: a 2D N=32 trajectory has n = 2048 unknowns = 16 KB per vector, so a CTA owns a whole trajectory:
 //   * iterate u and the current Krylov direction v_k live in shared memory (stencil neighbourhoods are read from there),
 //     the vector being orthogonalised w, the residual and the GMRES solution live in registers (8 rows per thread);
@@ -387,9 +393,18 @@ size_t ens_smem_bytes(const EnsParams& P) {
 }
 }  // namespace
 
+// The option sets the kernel implements exactly; everything else goes to the general driver (b200_ens_solve's sequential route).
+// Termination: the three AbsNorm modes on the inf-norm, with the Safe modes' step-stall window at its default of 32 (the
+// window is fixed in the kernel; a non-Safe mode has none, so its setting does not matter).  No wall-clock limit.
 int32_t b200i_ens_batched_supported(int32_t N, const b200_newton_opts* o) {
   if (2 * N * N > ET * NPT) return 0;
   if (o->jvp_mode != B200_JVP_EXACT || o->gmres.warm_start || o->gmres.restart > 0) return 0;
+  if (o->gmres.orth != B200_ORTH_MGS && o->gmres.orth != B200_ORTH_CGS2) return 0;
+  const int t = o->termination;
+  if (t != B200_TERM_ABS_NORM && t != B200_TERM_ABS_NORM_SAFE && t != B200_TERM_ABS_NORM_SAFE_BEST) return 0;
+  if (o->term_norm != B200_NORM_INF) return 0;
+  if (t != B200_TERM_ABS_NORM && o->term_max_stalled_steps != 0 && o->term_max_stalled_steps != 32) return 0;
+  if (o->maxtime > 0.0) return 0;
   return 1;
 }
 
@@ -412,7 +427,7 @@ int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double 
   int slab_cols = 512;
   if (const char* e = getenv("B200_ENS_BASIS_COLUMNS")) { const int v = atoi(e); if (v >= 2) slab_cols = v; }
   P.kcap = std::min(std::min(P.n, P.itmax), slab_cols);
-  P.passes = (o->gmres.orth == B200_ORTH_MGS) ? 1 : 2;  // MGS, or MGS applied twice (reorthogonalisation) for CGS2 / MGS2 requests
+  P.passes = (o->gmres.orth == B200_ORTH_MGS) ? 1 : 2;  // MGS, or MGS applied twice (reorthogonalisation) for CGS2
   P.term_mode = o->termination;
   P.forcing = o->forcing == B200_FORCING_EW2;
   P.ew_eta0 = o->ew_eta0; P.ew_eta_max = o->ew_eta_max; P.ew_gamma = o->ew_gamma; P.ew_alpha = o->ew_alpha;
