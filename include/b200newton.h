@@ -176,7 +176,7 @@ typedef struct b200_newton_opts {
   int32_t forcing;
   int32_t termination;
   int32_t store_trace;
-  int32_t fused_step; /* 1 = fuse u+=du, residual and norms into one kernel (default) ; 0 = separate ops */
+  int32_t fused_step; /* reserved and ignored: the update u += du, the residual and both norms always run as the two fused kernels */
   b200_gmres_opts gmres; /* atol/rtol <= 0 => inherit the nonlinear abstol/reltol (solve.jl:203) */
   /* Eisenstat-Walker forcing (eisenstat_walker.jl:18-30) */
   double ew_eta0, ew_eta_max, ew_gamma, ew_alpha, ew_safeguard_threshold;

@@ -13,8 +13,7 @@
 #include <math.h>
 #include <algorithm>
 #include <chrono>
-
-extern "C" int32_t b200_gmres_keep_hessenberg(b200_gmres* gm, int64_t capacity);
+#include <initializer_list>
 
 namespace {
 struct TermCache {  // NonlinearTerminationModeCache (termination_conditions.jl:60-98)
@@ -31,6 +30,13 @@ struct TermCache {  // NonlinearTerminationModeCache (termination_conditions.jl:
 struct TermQuant {
   double f_inf, f_norm, sum_norm, rel_viol;  // ||f||_inf ; internalnorm(f) ; internalnorm(f + u) ; #{ |f_i| > reltol |u_i + f_i| }
 };
+// The radius update scheme's constants (get_parameters, trust_region.jl:348-381): thresholds, factors and the shrink limit
+// hold for the solver's life; tp1..tp4 are the initial scheme parameters, restored by every reinit (Yuan and Fan mutate p1).
+struct TrParams {
+  double step_thr, shrink_thr, expand_thr, shrink_fac, expand_fac;
+  int max_shrink;
+  double tp1, tp2, tp3, tp4;
+};
 }  // namespace
 
 struct b200_newton {
@@ -40,7 +46,8 @@ struct b200_newton {
   int64_t n;
   double abstol, reltol;
   int maxiters;
-  double *u, *fu, *u_cache, *du, *xlin, *best_u;
+  std::vector<void*> allocs;  // every device buffer of the driver (dev_alloc), freed by b200_newton_destroy
+  double *u, *fu, *du, *xlin, *best_u;
   double *u_trial, *fu_trial, *Jdu, *JTfu, *du_c, *c1, *c2;
   b200_gmres* gm;
   b200_linop op;
@@ -55,18 +62,22 @@ struct b200_newton {
   b200_sparse_jac* sj;
   double* nzval;
   b200_sparse_lu* slu;  // LINSOLVE_SPARSE_LU: band factorisation of the assembled Jacobian
-  // LevenbergMarquardt: J'J + lambda D'D (factored in place), the running diagonal D'D, velocity / acceleration, previous velocity
+  // LevenbergMarquardt: J'J + lambda D'D (factored in place), the running diagonal D'D, velocity / acceleration, previous velocity, J' f
   double *lmA, *lm_dtd, *lm_v, *lm_a, *lm_vold, *lm_rhs;
+  double lm_lambda, lm_lambda_factor, lm_norm_v_old, lm_loss_old;
+  // Broyden family: the previous residual of the update rule (Klement's fu_cache) and of the reset test; the stored inverse
+  // (n x n, dense form only), J^-1 df, the rule's row vector w and rank-one column c; Klement's diagonal J (not inverted)
+  double *qn_dfu, *qn_dfu_reset, *qn_Jinv, *qn_Jdfu, *qn_w, *qn_c, *kl_J;
   int qn_since_du, qn_since_dfu, qn_nresets;  // Broyden: NoChangeInStateReset counters, resets so far
   double *lr_U, *lr_V, *lr_c;                // LimitedMemoryBroyden: J^-1 = lr_alpha I + U V' (n x lr_m each, circular), coefficient scratch
   int lr_m, lr_idx;
   double lr_alpha;
-  double lm_lambda, lm_lambda_factor, lm_norm_v_old, lm_loss_old;
   // state
   TermCache tc;
   b200_newton_result res;
   std::vector<b200_trace_rec> trace;
   int retcode, force_stop, make_new_jacobian, nsteps, have_factor, initialised;
+  TrParams trp;
   double trust_region, max_tr;
   int shrink_counter;
   double eta, rnorm, rnorm_prev;
@@ -150,9 +161,39 @@ int term_check(b200_newton* nw, const TermQuant& q, double du_norm, bool* new_be
   return 0;
 }
 
-int32_t alloc_vec(b200_ctx* ctx, int64_t n, double** p) {
-  CUDA_TRY(ctx, cudaMalloc(p, sizeof(double) * ((n + 1) & ~(int64_t)1)));
+// A device buffer of `count` elements that b200_newton_destroy frees; B200_ERR_NOMEM saying `what` when it does not fit.
+template <class T>
+int32_t dev_alloc(b200_newton* nw, T** p, size_t count, const char* what) {
+  if (cudaMalloc(p, sizeof(T) * count) != cudaSuccess) {
+    cudaGetLastError();
+    *p = nullptr;
+    return nw->ctx->fail(B200_ERR_NOMEM, what, __FILE__, __LINE__);
+  }
+  nw->allocs.push_back(*p);
   return B200_OK;
+}
+// n-vectors, padded to an even length
+int32_t dev_vecs(b200_newton* nw, std::initializer_list<double**> ps) {
+  for (double** p : ps) B200_TRY(dev_alloc(nw, p, (size_t)((nw->n + 1) & ~(int64_t)1), "newton_create: the driver's n-vectors do not fit in device memory"));
+  return B200_OK;
+}
+
+TrParams tr_params(const b200_newton_opts& o) {
+  const int sch = o.tr_scheme;
+  TrParams p;
+  p.step_thr = o.tr_step_threshold > 0 ? o.tr_step_threshold : (sch == B200_TR_HEI ? 0.0 : sch == B200_TR_YUAN ? 1.0 / 1000 : sch == B200_TR_BASTIN ? 1.0 / 20 : 1.0 / 10000);
+  p.shrink_thr = o.tr_shrink_threshold > 0 ? o.tr_shrink_threshold : (sch == B200_TR_HEI ? 0.0 : (sch == B200_TR_NLSOLVE || sch == B200_TR_BASTIN) ? 1.0 / 20 : 0.25);
+  p.expand_thr = o.tr_expand_threshold > 0 ? o.tr_expand_threshold : ((sch == B200_TR_NLSOLVE || sch == B200_TR_BASTIN) ? 0.9 : sch == B200_TR_HEI ? 0.0 : 0.75);
+  p.shrink_fac = o.tr_shrink_factor > 0 ? o.tr_shrink_factor : (sch == B200_TR_NLSOLVE ? 0.5 : sch == B200_TR_HEI ? 0.0 : sch == B200_TR_BASTIN ? 1.0 / 20 : 0.25);
+  p.expand_fac = o.tr_expand_factor > 0 ? o.tr_expand_factor : 2.0;
+  p.max_shrink = o.max_shrink_times > 0 ? o.max_shrink_times : 32;
+  p.tp1 = p.tp2 = p.tp3 = p.tp4 = 0.0;
+  if (sch == B200_TR_NLSOLVE) { p.tp1 = 0.5; }
+  else if (sch == B200_TR_HEI) { p.tp1 = 5.0; p.tp2 = 0.1; p.tp3 = 0.15; p.tp4 = 0.15; }
+  else if (sch == B200_TR_YUAN) { p.tp1 = 2.0; p.tp2 = 1.0 / 6; p.tp3 = 6.0; }
+  else if (sch == B200_TR_FAN) { p.tp1 = 0.1; p.tp2 = 0.25; p.tp3 = 12.0; p.tp4 = 1.0e18; }
+  else if (sch == B200_TR_BASTIN) { p.tp1 = 2.5; p.tp2 = 0.25; }
+  return p;
 }
 }  // namespace
 
@@ -179,19 +220,78 @@ void b200_newton_opts_default(b200_newton_opts* o) {
 int32_t b200_newton_destroy(b200_newton* nw) {
   B200_DEVICE_GUARD(nw ? nw->ctx : nullptr);
   if (!nw) return B200_OK;
-  b200_ctx* ctx = nw->ctx;
-  cudaStreamSynchronize(ctx->stream);
-  double* vecs[] = {nw->u, nw->fu, nw->u_cache, nw->du, nw->xlin, nw->best_u, nw->u_trial, nw->fu_trial, nw->Jdu, nw->JTfu, nw->du_c, nw->c1, nw->c2,
-                    nw->Jdense, nw->nzval, nw->lmA, nw->lm_dtd, nw->lm_v, nw->lm_a, nw->lm_vold, nw->lm_rhs, nw->lr_U, nw->lr_V, nw->lr_c};
-  for (double* v : vecs) if (v) cudaFree(v);
-  if (nw->ipiv) cudaFree(nw->ipiv);
-  if (nw->qr_work) cudaFree(nw->qr_work);
-  if (nw->qr_jpvt) cudaFree(nw->qr_jpvt);
+  cudaStreamSynchronize(nw->ctx->stream);
+  for (void* p : nw->allocs) cudaFree(p);
   if (nw->gm) b200_gmres_destroy(nw->gm);
   if (nw->mg) b200i_mg_destroy(nw->mg);
   if (nw->sj) b200_sparse_jac_destroy(nw->sj);
   if (nw->slu) b200_sparse_lu_destroy(nw->slu);
   delete nw;
+  return B200_OK;
+}
+
+// the buffers and sub-solvers b200_newton_create builds for the options; on failure the caller destroys the partial driver
+static int32_t newton_setup(b200_newton* nw) {
+  b200_ctx* ctx = nw->ctx;
+  b200_problem* prob = nw->prob;
+  const b200_newton_opts& o = nw->o;
+  const int64_t n = nw->n;
+  B200_TRY(dev_vecs(nw, {&nw->u, &nw->fu, &nw->du, &nw->xlin}));
+  if (term_is_best(o.termination)) B200_TRY(dev_vecs(nw, {&nw->best_u}));
+  if (o.globalization == B200_GLOBALIZATION_TRUST_REGION)
+    B200_TRY(dev_vecs(nw, {&nw->u_trial, &nw->fu_trial, &nw->Jdu, &nw->JTfu, &nw->du_c, &nw->c1, &nw->c2}));
+  if (o.globalization == B200_GLOBALIZATION_LINESEARCH) B200_TRY(dev_vecs(nw, {&nw->u_trial, &nw->fu_trial, &nw->Jdu}));
+  if (o.descent == B200_DESCENT_LEVENBERG_MARQUARDT) {
+    B200_TRY(dev_vecs(nw, {&nw->u_trial, &nw->fu_trial, &nw->Jdu, &nw->lm_dtd, &nw->lm_v, &nw->lm_a, &nw->lm_vold, &nw->lm_rhs}));
+    B200_TRY(dev_alloc(nw, &nw->lmA, (size_t)(n * n), "LevenbergMarquardt: J'J does not fit in device memory"));
+  }
+  if (o.descent == B200_DESCENT_BROYDEN) {
+    B200_TRY(dev_vecs(nw, {&nw->qn_dfu, &nw->qn_dfu_reset}));
+    if (o.qn_update_rule == B200_QN_UPDATE_KLEMENT) {
+      B200_TRY(dev_vecs(nw, {&nw->kl_J}));  // diagonal structure: nothing n x n
+    } else {
+      B200_TRY(dev_vecs(nw, {&nw->qn_Jdfu, &nw->qn_w, &nw->qn_c}));
+      if (o.qn_init_jacobian == B200_QN_INIT_LOW_RANK) {
+        nw->lr_m = std::max(1, std::min(o.qn_threshold > 0 ? o.qn_threshold : 10, nw->maxiters));  // threshold = min(threshold, maxiters)
+        const char* what = "LimitedMemoryBroyden: the low-rank factors do not fit in device memory";
+        B200_TRY(dev_alloc(nw, &nw->lr_U, (size_t)(n * nw->lr_m), what));
+        B200_TRY(dev_alloc(nw, &nw->lr_V, (size_t)(n * nw->lr_m), what));
+        B200_TRY(dev_alloc(nw, &nw->lr_c, (size_t)nw->lr_m, what));
+      } else {
+        B200_TRY(dev_alloc(nw, &nw->qn_Jinv, (size_t)(n * n), "Broyden: the stored inverse Jacobian (n x n) does not fit in device memory"));
+      }
+    }
+  }
+  nw->op.ctx = ctx; nw->op.n = n;
+  if (o.precond == B200_PRECOND_MULTIGRID_LEFT || o.precond == B200_PRECOND_MULTIGRID_RIGHT) B200_TRY(b200i_mg_create(prob, &nw->mg));
+  if (o.linsolve == B200_LINSOLVE_GMRES || o.linsolve == B200_LINSOLVE_SPARSE_GMRES) {
+    b200_gmres_opts g = o.gmres;
+    if (g.atol <= 0) g.atol = nw->abstol;  // linsolve_kwargs = (; abstol, reltol)   solve.jl:203
+    if (g.rtol <= 0) g.rtol = nw->reltol;
+    nw->o.gmres = g;
+    B200_TRY(b200_gmres_create(ctx, n, &g, &nw->gm));
+  }
+  if (o.linsolve == B200_LINSOLVE_GMRES) {
+    nw->op.kind = LINOP_PROBLEM; nw->op.prob = prob; nw->op.u = nw->u; nw->op.jvp_mode = o.jvp_mode;
+  } else if (o.linsolve == B200_LINSOLVE_DENSE_LU) {
+    B200_TRY(dev_alloc(nw, &nw->Jdense, (size_t)(n * n), "dense Jacobian does not fit in device memory"));
+    B200_TRY(dev_alloc(nw, &nw->ipiv, (size_t)n, "dense Jacobian does not fit in device memory"));
+  } else if (o.linsolve == B200_LINSOLVE_SPARSE_GMRES || o.linsolve == B200_LINSOLVE_SPARSE_LU) {
+    // jac_prototype + colouring once at init (jacobian.jl:286-353; colouring ext :13-28)
+    int64_t nnz = 0;
+    B200_TRY(b200_pattern_nnz(prob, &nnz));
+    std::vector<int64_t> colptr(n + 1), rowval(nnz), colors(n);
+    int64_t ncolors = 0;
+    B200_TRY(b200_pattern(prob, 1, colptr.data(), rowval.data()));
+    B200_TRY(b200_coloring_column(n, colptr.data(), rowval.data(), 1, B200_ORDER_LARGEST_FIRST, colors.data(), &ncolors));
+    B200_TRY(b200_sparse_jac_create(prob, colptr.data(), rowval.data(), 1, colors.data(), ncolors, &nw->sj));
+    B200_TRY(dev_alloc(nw, &nw->nzval, (size_t)nnz, "sparse Jacobian: the nonzero values do not fit in device memory"));
+    // sparse direct route (linsolve = nothing on a sparse prototype): symbolic phase once, like LinearSolve's cache
+    if (o.linsolve == B200_LINSOLVE_SPARSE_LU) B200_TRY(b200_sparse_lu_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->slu));
+    nw->op.kind = LINOP_SPARSE_JAC; nw->op.sj = nw->sj; nw->op.nzval = nw->nzval;
+  } else {
+    return ctx->fail(B200_ERR_INVALID, "unknown linsolve kind", __FILE__, __LINE__);
+  }
   return B200_OK;
 }
 
@@ -223,80 +323,9 @@ int32_t b200_newton_create(b200_problem* prob, const b200_newton_opts* opts, b20
   nw->abstol = opts->abstol > 0 ? opts->abstol : 3.0e-13;  // common_defaults.jl:44-48
   nw->reltol = opts->reltol > 0 ? opts->reltol : 3.0e-13;
   nw->maxiters = opts->maxiters > 0 ? opts->maxiters : 1000;
-  nw->u = nw->fu = nw->u_cache = nw->du = nw->xlin = nw->best_u = nullptr;
-  nw->u_trial = nw->fu_trial = nw->Jdu = nw->JTfu = nw->du_c = nw->c1 = nw->c2 = nullptr;
-  nw->qr_work = nullptr; nw->qr_jpvt = nullptr;
-  nw->lmA = nw->lm_dtd = nw->lm_v = nw->lm_a = nw->lm_vold = nw->lm_rhs = nullptr;
-  nw->lr_U = nw->lr_V = nw->lr_c = nullptr; nw->lr_m = nw->lr_idx = 0; nw->lr_alpha = 1.0;
-  nw->slu = nullptr; nw->mg = nullptr; nw->gm = nullptr; nw->Jdense = nullptr; nw->ipiv = nullptr; nw->sj = nullptr; nw->nzval = nullptr;
-  nw->initialised = 0;
-  const int64_t n = nw->n;
-  int32_t s = B200_OK;
-  auto A = [&](double** p) { if (s == B200_OK) s = alloc_vec(ctx, n, p); };
-  A(&nw->u); A(&nw->fu); A(&nw->u_cache); A(&nw->du); A(&nw->xlin);
-  if (term_is_best(opts->termination)) A(&nw->best_u);
-  if (opts->globalization == B200_GLOBALIZATION_TRUST_REGION) {
-    A(&nw->u_trial); A(&nw->fu_trial); A(&nw->Jdu); A(&nw->JTfu); A(&nw->du_c); A(&nw->c1); A(&nw->c2);
-  }
-  if (opts->globalization == B200_GLOBALIZATION_LINESEARCH) { A(&nw->u_trial); A(&nw->fu_trial); A(&nw->Jdu); }
-  if (opts->descent == B200_DESCENT_LEVENBERG_MARQUARDT) {
-    A(&nw->u_trial); A(&nw->fu_trial); A(&nw->Jdu); A(&nw->lm_dtd); A(&nw->lm_v); A(&nw->lm_a); A(&nw->lm_vold); A(&nw->lm_rhs);
-    if (s == B200_OK && cudaMalloc(&nw->lmA, sizeof(double) * n * n) != cudaSuccess) { cudaGetLastError(); s = ctx->fail(B200_ERR_NOMEM, "LevenbergMarquardt: J'J does not fit in device memory", __FILE__, __LINE__); }
-  }
-  if (opts->descent == B200_DESCENT_BROYDEN) {  // the stored inverse and the update rule's / reset condition's vectors share the LM slots
-    A(&nw->lm_dtd); A(&nw->lm_v); A(&nw->lm_a); A(&nw->lm_vold); A(&nw->lm_rhs);
-    if (opts->qn_update_rule == B200_QN_UPDATE_KLEMENT) {
-      // diagonal structure: the approximate Jacobian is the n-vector lm_dtd, the rule's residual cache lm_v — nothing n x n
-    } else if (opts->qn_init_jacobian == B200_QN_INIT_LOW_RANK) {
-      nw->lr_m = std::max(1, std::min(opts->qn_threshold > 0 ? opts->qn_threshold : 10, nw->maxiters));  // threshold = min(threshold, maxiters)
-      if (s == B200_OK && (cudaMalloc(&nw->lr_U, sizeof(double) * n * nw->lr_m) != cudaSuccess || cudaMalloc(&nw->lr_V, sizeof(double) * n * nw->lr_m) != cudaSuccess ||
-                           cudaMalloc(&nw->lr_c, sizeof(double) * nw->lr_m) != cudaSuccess)) {
-        cudaGetLastError();
-        s = ctx->fail(B200_ERR_NOMEM, "LimitedMemoryBroyden: the low-rank factors do not fit in device memory", __FILE__, __LINE__);
-      }
-    } else if (s == B200_OK && cudaMalloc(&nw->lmA, sizeof(double) * n * n) != cudaSuccess) { cudaGetLastError(); s = ctx->fail(B200_ERR_NOMEM, "Broyden: the stored inverse Jacobian (n x n) does not fit in device memory", __FILE__, __LINE__); }
-  }
+  nw->trp = tr_params(*opts);
+  const int32_t s = newton_setup(nw);
   if (s != B200_OK) { b200_newton_destroy(nw); return s; }
-  memset(&nw->op, 0, sizeof(nw->op));
-  nw->op.ctx = ctx; nw->op.n = n;
-  if (opts->precond == B200_PRECOND_MULTIGRID_LEFT || opts->precond == B200_PRECOND_MULTIGRID_RIGHT) {
-    s = b200i_mg_create(prob, &nw->mg);
-    if (s != B200_OK) { b200_newton_destroy(nw); return s; }
-  }
-  if (opts->linsolve == B200_LINSOLVE_GMRES || opts->linsolve == B200_LINSOLVE_SPARSE_GMRES) {
-    b200_gmres_opts g = opts->gmres;
-    if (g.atol <= 0) g.atol = nw->abstol;  // linsolve_kwargs = (; abstol, reltol)   solve.jl:203
-    if (g.rtol <= 0) g.rtol = nw->reltol;
-    nw->o.gmres = g;
-    s = b200_gmres_create(ctx, n, &g, &nw->gm);
-    if (s != B200_OK) { b200_newton_destroy(nw); return s; }
-  }
-  if (opts->linsolve == B200_LINSOLVE_GMRES) {
-    nw->op.kind = LINOP_PROBLEM; nw->op.prob = prob; nw->op.u = nw->u; nw->op.jvp_mode = opts->jvp_mode;
-  } else if (opts->linsolve == B200_LINSOLVE_DENSE_LU) {
-    if (cudaMalloc(&nw->Jdense, sizeof(double) * n * n) != cudaSuccess || cudaMalloc(&nw->ipiv, sizeof(int64_t) * n) != cudaSuccess) {
-      cudaGetLastError();
-      b200_newton_destroy(nw);
-      return ctx->fail(B200_ERR_NOMEM, "dense Jacobian does not fit in device memory", __FILE__, __LINE__);
-    }
-  } else if (opts->linsolve == B200_LINSOLVE_SPARSE_GMRES || opts->linsolve == B200_LINSOLVE_SPARSE_LU) {
-    // jac_prototype + colouring once at init (jacobian.jl:286-353; colouring ext :13-28)
-    int64_t nnz = 0;
-    s = b200_pattern_nnz(prob, &nnz);
-    std::vector<int64_t> colptr(n + 1), rowval(nnz), colors(n);
-    int64_t ncolors = 0;
-    if (s == B200_OK) s = b200_pattern(prob, 1, colptr.data(), rowval.data());
-    if (s == B200_OK) s = b200_coloring_column(n, colptr.data(), rowval.data(), 1, B200_ORDER_LARGEST_FIRST, colors.data(), &ncolors);
-    if (s == B200_OK) s = b200_sparse_jac_create(prob, colptr.data(), rowval.data(), 1, colors.data(), ncolors, &nw->sj);
-    if (s == B200_OK && cudaMalloc(&nw->nzval, sizeof(double) * nnz) != cudaSuccess) { cudaGetLastError(); s = B200_ERR_NOMEM; }
-    // sparse direct route (linsolve = nothing on a sparse prototype): symbolic phase once, like LinearSolve's cache
-    if (s == B200_OK && opts->linsolve == B200_LINSOLVE_SPARSE_LU) s = b200_sparse_lu_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->slu);
-    if (s != B200_OK) { b200_newton_destroy(nw); return s; }
-    nw->op.kind = LINOP_SPARSE_JAC; nw->op.sj = nw->sj; nw->op.nzval = nw->nzval;
-  } else {
-    b200_newton_destroy(nw);
-    return ctx->fail(B200_ERR_INVALID, "unknown linsolve kind", __FILE__, __LINE__);
-  }
   *out = nw;
   return B200_OK;
 }
@@ -310,7 +339,6 @@ int32_t b200_newton_reinit(b200_newton* nw, const double* u0_dev) {
   if (u0_dev != nw->u) CUDA_TRY(ctx, cudaMemcpyAsync(nw->u, u0_dev, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
   CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 4, ctx->stream));
   B200_TRY(b200i_residual_norm(nw->prob, nw->u, nw->fu, ctx->d_scalars));  // evaluate_f(prob,u): nf is NOT bumped (solve.jl:194)
-  CUDA_TRY(ctx, cudaMemcpyAsync(nw->u_cache, nw->u, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
   CUDA_TRY(ctx, cudaMemsetAsync(nw->du, 0, sizeof(double) * n, ctx->stream));  // descent caches start with a defined du
   if (nw->best_u) CUDA_TRY(ctx, cudaMemcpyAsync(nw->best_u, nw->u, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
   B200_TRY(b200i_fetch_scalars(ctx, 1));
@@ -344,12 +372,7 @@ int32_t b200_newton_reinit(b200_newton* nw, const double* u0_dev) {
     B200_TRY(h_nrm2(nw, nw->fu, &fu_norm));
     B200_TRY(h_nrm2(nw, nw->u, &u0_norm));
     B200_TRY(b200_extrema(ctx, n, nw->u, &umin, &umax));
-    nw->tp1 = nw->tp2 = nw->tp3 = nw->tp4 = 0.0;
-    if (sch == B200_TR_NLSOLVE) { nw->tp1 = 0.5; }
-    else if (sch == B200_TR_HEI) { nw->tp1 = 5.0; nw->tp2 = 0.1; nw->tp3 = 0.15; nw->tp4 = 0.15; }
-    else if (sch == B200_TR_YUAN) { nw->tp1 = 2.0; nw->tp2 = 1.0 / 6; nw->tp3 = 6.0; }
-    else if (sch == B200_TR_FAN) { nw->tp1 = 0.1; nw->tp2 = 0.25; nw->tp3 = 12.0; nw->tp4 = 1.0e18; }
-    else if (sch == B200_TR_BASTIN) { nw->tp1 = 2.5; nw->tp2 = 0.25; }
+    nw->tp1 = nw->trp.tp1; nw->tp2 = nw->trp.tp2; nw->tp3 = nw->trp.tp3; nw->tp4 = nw->trp.tp4;
     if (o.tr_max_trust_radius > 0) nw->max_tr = o.tr_max_trust_radius;  // max_trust_radius  :330-337
     else nw->max_tr = (sch == B200_TR_SIMPLE || sch == B200_TR_NOCEDAL_WRIGHT) ? std::max(fu_norm, umax - umin) : INFINITY;  // Hei, Yuan, Fan, NLsolve, Bastin: unbounded
     if (o.tr_initial_trust_radius > 0) nw->trust_region = o.tr_initial_trust_radius;  // initial_trust_radius  :339-346
@@ -378,8 +401,8 @@ int32_t b200_newton_reinit(b200_newton* nw, const double* u0_dev) {
     nw->lm_loss_old = INFINITY;
   }
   if (o.descent == B200_DESCENT_BROYDEN) {  // BroydenUpdateRuleCache.dfu = copy(fu); NoChangeInStateResetCache.dfu = copy(fu); counters 0
-    B200_TRY(b200_copy(ctx, n, nw->fu, nw->lm_v));
-    B200_TRY(b200_copy(ctx, n, nw->fu, nw->lm_a));
+    B200_TRY(b200_copy(ctx, n, nw->fu, nw->qn_dfu));
+    B200_TRY(b200_copy(ctx, n, nw->fu, nw->qn_dfu_reset));
     B200_TRY(b200_fill(ctx, n, 0.0, nw->du));
     nw->qn_since_du = nw->qn_since_dfu = nw->qn_nresets = 0;
   }
@@ -390,6 +413,51 @@ int32_t b200_newton_reinit(b200_newton* nw, const double* u0_dev) {
     nw->rnorm_prev = nw->rnorm;
   }
   nw->initialised = 1;
+  return B200_OK;
+}
+
+// u += a du ; fu = f(u), with ||du||_2^2 and ||fu||_inf from the two kernels' epilogues, fetched together (solve.jl:403-407, 436-445)
+static int32_t update_u(b200_newton* nw, double a, double* objective, double* du_norm) {
+  b200_ctx* ctx = nw->ctx;
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
+  B200_TRY(b200i_axpy_norm(ctx, nw->n, a, nw->du, nw->u, ctx->d_scalars + 1));
+  B200_TRY(b200i_residual_norm(nw->prob, nw->u, nw->fu, ctx->d_scalars));
+  nw->res.nf += 1;
+  B200_TRY(b200i_fetch_scalars(ctx, 2));
+  *objective = ctx->h_scalars[0];
+  *du_norm = sqrt(ctx->h_scalars[1]);
+  return B200_OK;
+}
+
+// u_trial = u + a d
+static int32_t trial_point(b200_newton* nw, double a, const double* d) {
+  B200_TRY(b200_copy(nw->ctx, nw->n, nw->u, nw->u_trial));
+  return b200_axpy(nw->ctx, nw->n, a, d, nw->u_trial);
+}
+
+// the trial point becomes the iterate: copyto!(cache.u, u_new) as a pointer swap
+static void accept_trial(b200_newton* nw) {
+  std::swap(nw->u, nw->u_trial);
+  std::swap(nw->fu, nw->fu_trial);
+  nw->op.u = nw->u;
+}
+
+// The end of every step: check_and_update! (the termination test on the iterate with ||f||_inf = objective, the best
+// iterate), then update_trace!.  `t` carries the step's own fields (accepted, lin_*, trust_radius); LevenbergMarquardt
+// skips the test (check = false) when its descent rejected the step.
+static int32_t step_end(b200_newton* nw, double objective, double du_norm, b200_trace_rec t, bool check = true) {
+  if (check) {
+    nw->fnorm_inf = objective;
+    bool new_best = false;
+    TermQuant tq;
+    B200_TRY(term_quantities(nw, nw->fu, nw->u, objective, &tq));
+    if (term_check(nw, tq, du_norm, &new_best)) { nw->retcode = nw->tc.retcode; nw->force_stop = 1; }
+    if (new_best && nw->best_u) CUDA_TRY(nw->ctx, cudaMemcpyAsync(nw->best_u, nw->u, sizeof(double) * nw->n, cudaMemcpyDeviceToDevice, nw->ctx->stream));
+  }
+  if (nw->o.store_trace) {
+    t.iter = nw->nsteps + 1; t.fnorm_inf = objective; t.step_norm2 = du_norm;
+    nw->trace.push_back(t);
+  }
   return B200_OK;
 }
 
@@ -429,8 +497,7 @@ static int32_t lm_step(b200_newton* nw) {
   B200_TRY(h_nrm2(nw, nw->lm_v, &norm_v));
   if (!o.lm_disable_geodesic) {
     // geodesic acceleration: fu_cache = (2/h) ((f(u + h v) - f(u)) / h - J v) ; a = -(A^-1 J' fu_cache) with the same factorisation
-    B200_TRY(b200_copy(ctx, n, nw->u, nw->u_trial));
-    B200_TRY(b200_axpy(ctx, n, h, nw->lm_v, nw->u_trial));
+    B200_TRY(trial_point(nw, h, nw->lm_v));
     B200_TRY(b200_residual(nw->prob, nw->u_trial, nw->fu_trial));              // evaluate_f!! inside the descent: NLStats.nf is not bumped
     B200_TRY(b200_gemv(ctx, 0, n, n, nw->Jdense, n, nw->lm_v, nw->Jdu));        // J v
     B200_TRY(b200_axpy(ctx, n, -1.0, nw->fu, nw->fu_trial));
@@ -448,17 +515,15 @@ static int32_t lm_step(b200_newton* nw) {
       descent_ok = 0;  // the step is not taken; du keeps its previous value (geodesic_acceleration.jl:131-133)
     }
   } else {
-    nw->res.nsolve += 0;
     B200_TRY(b200_copy(ctx, n, nw->lm_v, nw->du));
   }
+  nw->make_new_jacobian = 0;
   if (descent_ok) {
-    nw->make_new_jacobian = 1;
     // ---- LevenbergMarquardtTrustRegion: beta = cos(v, v_old); accept iff (1 - beta)^b_uphill * ||f(u + du)|| <= loss_old
     double vdot;
     B200_TRY(h_dot(nw, nw->lm_v, nw->lm_vold, &vdot));
     const double beta = vdot / (norm_v * nw->lm_norm_v_old);
-    B200_TRY(b200_copy(ctx, n, nw->u, nw->u_trial));
-    B200_TRY(b200_axpy(ctx, n, 1.0, nw->du, nw->u_trial));
+    B200_TRY(trial_point(nw, 1.0, nw->du));
     CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
     B200_TRY(b200i_residual_norm(nw->prob, nw->u_trial, nw->fu_trial, ctx->d_scalars));
     nw->res.nf += 1;
@@ -468,36 +533,34 @@ static int32_t lm_step(b200_newton* nw) {
     B200_TRY(h_nrm2(nw, nw->fu_trial, &loss));
     tr_ok = (pow(1.0 - beta, b_uphill) * loss <= nw->lm_loss_old) ? 1 : 0;     // loss_old is never updated by the reference (stays Inf)
     if (tr_ok) {
+      nw->make_new_jacobian = 1;
       nw->lm_norm_v_old = norm_v;
       B200_TRY(b200_copy(ctx, n, nw->lm_v, nw->lm_vold));
       B200_TRY(h_nrm2(nw, nw->du, &du_norm));
-      std::swap(nw->u, nw->u_trial);
-      std::swap(nw->fu, nw->fu_trial);
+      accept_trial(nw);
       objective = trial_inf;
       accepted = 1;
-    } else {
-      nw->make_new_jacobian = 0;
     }
-    nw->fnorm_inf = objective;
-    bool new_best = false;
-    TermQuant tq;
-    B200_TRY(term_quantities(nw, nw->fu, nw->u, objective, &tq));
-    if (term_check(nw, tq, du_norm, &new_best)) { nw->retcode = nw->tc.retcode; nw->force_stop = 1; }
-    if (new_best && nw->best_u) CUDA_TRY(ctx, cudaMemcpyAsync(nw->best_u, nw->u, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-  } else {
-    nw->make_new_jacobian = 0;
   }
-  if (o.store_trace) {
-    b200_trace_rec t;
-    memset(&t, 0, sizeof(t));
-    t.iter = nw->nsteps + 1; t.accepted = accepted; t.fnorm_inf = objective; t.step_norm2 = du_norm; t.trust_radius = nw->lm_lambda;  // the damping USED by this step
-    t.lin_status = descent_ok;
-    nw->trace.push_back(t);
-  }
+  b200_trace_rec t = {};
+  t.accepted = accepted; t.lin_status = descent_ok; t.trust_radius = nw->lm_lambda;  // the damping USED by this step
+  B200_TRY(step_end(nw, objective, du_norm, t, descent_ok));
   // callback_into_cache! (levenberg_marquardt.jl:176-185): lambda shrinks after a step both the descent and the trust region accepted
   if (descent_ok && tr_ok) nw->lm_lambda_factor = 1.0 / dec;
   nw->lm_lambda *= nw->lm_lambda_factor;
   nw->lm_lambda_factor = inc;
+  return B200_OK;
+}
+
+// Utils.initial_jacobian_scaling_alpha(alpha, u, fu, L2) of Broyden, LimitedMemoryBroyden and Klement: the given alpha, else
+// 2 ||f|| / max(||u||, 1); 1 below ||f|| = 1e-5
+static int32_t qn_initial_alpha(b200_newton* nw, double* alpha) {
+  *alpha = nw->o.qn_alpha;
+  if (*alpha > 0) return B200_OK;
+  double fn, un;
+  B200_TRY(h_nrm2(nw, nw->fu, &fn));
+  B200_TRY(h_nrm2(nw, nw->u, &un));
+  *alpha = (fn < 1.0e-5) ? 1.0 : (2.0 * fn) / std::max(un, 1.0);
   return B200_OK;
 }
 
@@ -510,7 +573,6 @@ static int32_t lm_step(b200_newton* nw) {
 static int32_t broyden_init_inverse(b200_newton* nw) {
   b200_ctx* ctx = nw->ctx;
   const int64_t n = nw->n;
-  double* Jinv = nw->lmA;
   if (nw->o.qn_init_jacobian == B200_QN_INIT_TRUE_JACOBIAN) {  // J^-1 = J \ I through the LU (Utils.linsolve_identity!!)
     nw->res.njacs += 1;
     B200_TRY(b200_dense_jac_fill(nw->prob, nw->u, nw->Jdense, n));
@@ -518,30 +580,25 @@ static int32_t broyden_init_inverse(b200_newton* nw) {
     nw->res.nfactors += 1;
     B200_TRY(b200_getrf(ctx, n, nw->Jdense, n, nw->ipiv, &info));
     if (info != 0) { nw->retcode = B200_RC_INTERNAL_LINSOLVE_FAILED; nw->force_stop = 1; return B200_OK; }
-    B200_TRY(b200i_scaled_identity(ctx, n, Jinv, n, 1.0));
-    B200_TRY(b200_getrs(ctx, n, n, nw->Jdense, n, nw->ipiv, Jinv, n));
+    B200_TRY(b200i_scaled_identity(ctx, n, nw->qn_Jinv, n, 1.0));
+    B200_TRY(b200_getrs(ctx, n, n, nw->Jdense, n, nw->ipiv, nw->qn_Jinv, n));
     return B200_OK;
   }
-  double alpha = nw->o.qn_alpha;
-  if (!(alpha > 0)) {  // Utils.initial_jacobian_scaling_alpha(nothing, u, fu, L2): 2 ||f|| / max(||u||, 1); 1 below ||f|| = 1e-5
-    double fn, un;
-    B200_TRY(h_nrm2(nw, nw->fu, &fn));
-    B200_TRY(h_nrm2(nw, nw->u, &un));
-    alpha = (fn < 1.0e-5) ? 1.0 : (2.0 * fn) / std::max(un, 1.0);
-  }
+  double alpha;
+  B200_TRY(qn_initial_alpha(nw, &alpha));
   if (nw->o.qn_init_jacobian == B200_QN_INIT_LOW_RANK) {  // BroydenLowRankJacobian: idx = 0, alpha = inv(scaling)   initialization.jl:176-199
     nw->lr_idx = 0;
     nw->lr_alpha = 1.0 / alpha;
     return B200_OK;
   }
-  return b200i_scaled_identity(ctx, n, Jinv, n, 1.0 / alpha);
+  return b200i_scaled_identity(ctx, n, nw->qn_Jinv, n, 1.0 / alpha);
 }
 
 // y = J^-1 x (transpose = 0) or J^-T x (1): the dense stored inverse, or alpha x + U (V' x) resp. alpha x + V (U' x) for the low-rank form
 static int32_t broyden_apply(b200_newton* nw, int transpose, const double* x, double* y) {
   b200_ctx* ctx = nw->ctx;
   const int64_t n = nw->n;
-  if (nw->o.qn_init_jacobian != B200_QN_INIT_LOW_RANK) return b200_gemv(ctx, transpose, n, n, nw->lmA, n, x, y);
+  if (nw->o.qn_init_jacobian != B200_QN_INIT_LOW_RANK) return b200_gemv(ctx, transpose, n, n, nw->qn_Jinv, n, x, y);
   const int k = std::min(nw->lr_idx, nw->lr_m);
   if (k > 0) {
     const double *L = transpose ? nw->lr_V : nw->lr_U, *R = transpose ? nw->lr_U : nw->lr_V;
@@ -565,55 +622,35 @@ static int32_t broyden_count(b200_newton* nw, const double* x, const double* y, 
 static int32_t klement_step(b200_newton* nw) {
   b200_ctx* ctx = nw->ctx;
   const int64_t n = nw->n;
-  const b200_newton_opts& o = nw->o;
-  double *J = nw->lm_dtd, *fu_cache = nw->lm_v;
-  const int max_resets = o.qn_max_resets > 0 ? o.qn_max_resets : 100;
+  const int max_resets = nw->o.qn_max_resets > 0 ? nw->o.qn_max_resets : 100;
   auto init_diag = [&]() -> int32_t {
-    double alpha = o.qn_alpha;
-    if (!(alpha > 0)) {
-      double fn, un;
-      B200_TRY(h_nrm2(nw, nw->fu, &fn));
-      B200_TRY(h_nrm2(nw, nw->u, &un));
-      alpha = (fn < 1.0e-5) ? 1.0 : (2.0 * fn) / std::max(un, 1.0);
-    }
-    return b200_fill(ctx, n, alpha, J);   // J = one.(fu) .* alpha, NOT inverted (store_inverse_jacobian = false)
+    double alpha;
+    B200_TRY(qn_initial_alpha(nw, &alpha));
+    return b200_fill(ctx, n, alpha, nw->kl_J);   // J = one.(fu) .* alpha, NOT inverted (store_inverse_jacobian = false)
   };
   int reset = 0;
   if (nw->nsteps == 0) {
     B200_TRY(init_diag());
   } else {
     double zeros;  // IllConditionedJacobianReset on a Diagonal: any(iszero, diag(J))
-    B200_TRY(broyden_count(nw, J, nullptr, 0.0, &zeros));
+    B200_TRY(broyden_count(nw, nw->kl_J, nullptr, 0.0, &zeros));
     if (zeros > 0) {
       reset = 1;
       if (++nw->qn_nresets >= max_resets) { nw->retcode = B200_RC_CONVERGENCE_FAILURE; nw->force_stop = 1; return B200_OK; }
       B200_TRY(init_diag());
     }
   }
-  B200_TRY(b200i_klement_descent(ctx, n, J, nw->fu, nw->du));
-  CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
-  B200_TRY(b200i_axpy_norm(ctx, n, 1.0, nw->du, nw->u, ctx->d_scalars + 1));
-  B200_TRY(b200i_residual_norm(nw->prob, nw->u, nw->fu, ctx->d_scalars));
-  nw->res.nf += 1;
+  B200_TRY(b200i_klement_descent(ctx, n, nw->kl_J, nw->fu, nw->du));
+  double objective, du_norm;
+  B200_TRY(update_u(nw, 1.0, &objective, &du_norm));
   nw->res.nsolve += 1;   // the diagonal system goes through NativeJLLinearSolveCache (linear_solve.jl:130-134): nsolve and nfactors both +1
   nw->res.nfactors += 1;
-  B200_TRY(b200i_fetch_scalars(ctx, 2));
-  const double objective = ctx->h_scalars[0], du_norm = sqrt(ctx->h_scalars[1]);
-  nw->fnorm_inf = objective;
   nw->bytes += 8.0 * (double)n * 8.0;
-  bool new_best = false;
-  TermQuant tq;
-  B200_TRY(term_quantities(nw, nw->fu, nw->u, objective, &tq));
-  if (term_check(nw, tq, du_norm, &new_best)) { nw->retcode = nw->tc.retcode; nw->force_stop = 1; }
-  if (new_best && nw->best_u) CUDA_TRY(ctx, cudaMemcpyAsync(nw->best_u, nw->u, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (o.store_trace) {
-    b200_trace_rec t;
-    memset(&t, 0, sizeof(t));
-    t.iter = nw->nsteps + 1; t.accepted = 1; t.fnorm_inf = objective; t.step_norm2 = du_norm; t.lin_status = reset;
-    nw->trace.push_back(t);
-  }
+  b200_trace_rec t = {};
+  t.accepted = 1; t.lin_status = reset;
+  B200_TRY(step_end(nw, objective, du_norm, t));
   if (nw->force_stop) return B200_OK;
-  return b200i_klement_update(ctx, n, J, nw->fu, fu_cache, nw->du);
+  return b200i_klement_update(ctx, n, nw->kl_J, nw->fu, nw->qn_dfu, nw->du);
 }
 
 static int32_t broyden_step(b200_newton* nw) {
@@ -621,7 +658,6 @@ static int32_t broyden_step(b200_newton* nw) {
   b200_ctx* ctx = nw->ctx;
   const int64_t n = nw->n;
   const b200_newton_opts& o = nw->o;
-  double *Jinv = nw->lmA, *dfu_rule = nw->lm_v, *dfu_reset = nw->lm_a, *Jd = nw->lm_vold, *w = nw->lm_rhs, *c = nw->lm_dtd;
   const double tol = o.qn_reset_tolerance > 0 ? o.qn_reset_tolerance : 1.8189894035458565e-12;  // eps^(3/4)
   const int max_resets = o.qn_max_resets > 0 ? o.qn_max_resets : 100;
   int reset = 0;
@@ -638,13 +674,13 @@ static int32_t broyden_step(b200_newton* nw) {
       nw->qn_since_du = nw->qn_since_dfu = 0;
     }
     if (!reset) {
-      B200_TRY(broyden_count(nw, nw->fu, dfu_reset, tol, &cnt));
+      B200_TRY(broyden_count(nw, nw->fu, nw->qn_dfu_reset, tol, &cnt));
       if (cnt > 0) {
         if (++nw->qn_since_dfu >= 3) { nw->qn_since_dfu = nw->qn_since_du = 0; reset = 1; }
       } else {
         nw->qn_since_dfu = nw->qn_since_du = 0;
       }
-      B200_TRY(b200_copy(ctx, n, nw->fu, dfu_reset));
+      B200_TRY(b200_copy(ctx, n, nw->fu, nw->qn_dfu_reset));
     }
     if (reset) {
       if (++nw->qn_nresets >= max_resets) { nw->retcode = B200_RC_CONVERGENCE_FAILURE; nw->force_stop = 1; return B200_OK; }
@@ -655,45 +691,34 @@ static int32_t broyden_step(b200_newton* nw) {
   // ---- NewtonDescent on the stored inverse: du = -(J^-1 f) ; u += du ; f = f(u)
   B200_TRY(broyden_apply(nw, 0, nw->fu, nw->du));
   B200_TRY(b200_scal(ctx, n, -1.0, nw->du));
-  CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
-  B200_TRY(b200i_axpy_norm(ctx, n, 1.0, nw->du, nw->u, ctx->d_scalars + 1));
-  B200_TRY(b200i_residual_norm(nw->prob, nw->u, nw->fu, ctx->d_scalars));
-  nw->res.nf += 1;
-  B200_TRY(b200i_fetch_scalars(ctx, 2));
-  const double objective = ctx->h_scalars[0], du_norm = sqrt(ctx->h_scalars[1]);
-  nw->fnorm_inf = objective;
+  double objective, du_norm;
+  B200_TRY(update_u(nw, 1.0, &objective, &du_norm));
   const double pass_bytes = (o.qn_init_jacobian == B200_QN_INIT_LOW_RANK) ? 16.0 * (double)n * std::min(nw->lr_idx, nw->lr_m) : 8.0 * (double)n * (double)n;  // one product with the stored inverse
   nw->bytes += pass_bytes;
-  bool new_best = false;
-  TermQuant tq;
-  B200_TRY(term_quantities(nw, nw->fu, nw->u, objective, &tq));
-  if (term_check(nw, tq, du_norm, &new_best)) { nw->retcode = nw->tc.retcode; nw->force_stop = 1; }
-  if (new_best && nw->best_u) CUDA_TRY(ctx, cudaMemcpyAsync(nw->best_u, nw->u, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (o.store_trace) {
-    b200_trace_rec t;
-    memset(&t, 0, sizeof(t));
-    t.iter = nw->nsteps + 1; t.accepted = 1; t.fnorm_inf = objective; t.step_norm2 = du_norm; t.lin_status = reset;  // lin_status: J^-1 was re-initialised before this step
-    nw->trace.push_back(t);
-  }
+  b200_trace_rec t = {};
+  t.accepted = 1; t.lin_status = reset;  // lin_status: J^-1 was re-initialised before this step
+  B200_TRY(step_end(nw, objective, du_norm, t));
   if (nw->force_stop) return B200_OK;  // the reference skips the update once the step has stopped the solve
   // ---- update rule
-  B200_TRY(b200_axpby(ctx, n, 1.0, nw->fu, -1.0, dfu_rule));             // dfu = fu - dfu
-  B200_TRY(broyden_apply(nw, 0, dfu_rule, Jd));                          // J^-1 dfu
+  double* dfu = nw->qn_dfu;
+  B200_TRY(b200_axpby(ctx, n, 1.0, nw->fu, -1.0, dfu));                  // dfu = fu - dfu
+  B200_TRY(broyden_apply(nw, 0, dfu, nw->qn_Jdfu));                      // J^-1 dfu
   double denom;
   const double* rmul;
   if (o.qn_update_rule == B200_QN_UPDATE_GOOD_BROYDEN) {
-    B200_TRY(broyden_apply(nw, 1, nw->du, w));                           // J^-T du
-    B200_TRY(h_dot(nw, nw->du, Jd, &denom));
-    rmul = w;
+    B200_TRY(broyden_apply(nw, 1, nw->du, nw->qn_w));                    // J^-T du
+    B200_TRY(h_dot(nw, nw->du, nw->qn_Jdfu, &denom));
+    rmul = nw->qn_w;
   } else {
     double nd;
-    B200_TRY(h_nrm2(nw, dfu_rule, &nd));
+    B200_TRY(h_nrm2(nw, dfu, &nd));
     denom = nd * nd;
-    rmul = dfu_rule;
+    rmul = dfu;
   }
   const double inv = 1.0 / (denom == 0.0 ? 1.0e-5 : denom);
+  double* c = nw->qn_c;
   B200_TRY(b200_copy(ctx, n, nw->du, c));
-  B200_TRY(b200_axpy(ctx, n, -1.0, Jd, c));
+  B200_TRY(b200_axpy(ctx, n, -1.0, nw->qn_Jdfu, c));
   B200_TRY(b200_scal(ctx, n, inv, c));                                   // (du - J^-1 dfu) / denom
   if (o.qn_init_jacobian == B200_QN_INIT_LOW_RANK) {                      // mul!(J, u, v', true, true): the pair goes into slot idx mod m
     const int slot = nw->lr_idx % nw->lr_m;
@@ -701,343 +726,344 @@ static int32_t broyden_step(b200_newton* nw) {
     B200_TRY(b200_copy(ctx, n, rmul, nw->lr_V + (int64_t)slot * n));
     nw->lr_idx += 1;
   } else {
-    B200_TRY(b200i_ger(ctx, n, Jinv, n, c, rmul));                       // J^-1 += c rmul'
+    B200_TRY(b200i_ger(ctx, n, nw->qn_Jinv, n, c, rmul));                // J^-1 += c rmul'
   }
-  B200_TRY(b200_copy(ctx, n, nw->fu, dfu_rule));
+  B200_TRY(b200_copy(ctx, n, nw->fu, dfu));
   nw->bytes += pass_bytes * (o.qn_update_rule == B200_QN_UPDATE_GOOD_BROYDEN ? 4.0 : 3.0);
   return B200_OK;
 }
 
-static int32_t newton_step_inner(b200_newton* nw) {
-  if (nw->o.descent == B200_DESCENT_LEVENBERG_MARQUARDT) return lm_step(nw);
-  if (nw->o.descent == B200_DESCENT_BROYDEN) return broyden_step(nw);
+static bool krylov_linsolve(const b200_newton_opts& o) { return o.linsolve == B200_LINSOLVE_GMRES || o.linsolve == B200_LINSOLVE_SPARSE_GMRES; }
+
+// J = cache.jac_cache(u) when the step asks for one (solve.jl:338-344); *fresh: the step works with a new Jacobian
+static int32_t refresh_jacobian(b200_newton* nw, bool* fresh) {
+  *fresh = nw->make_new_jacobian != 0;
+  if (!*fresh || nw->o.linsolve == B200_LINSOLVE_GMRES) return B200_OK;  // matrix-free: nothing to assemble
+  nw->res.njacs += 1;
+  nw->have_factor = 0;
+  if (nw->o.linsolve == B200_LINSOLVE_DENSE_LU) return b200_dense_jac_fill(nw->prob, nw->u, nw->Jdense, nw->n);  // written straight into the LU workspace (K10: no copyto!)
+  return b200_sparse_jac_fill(nw->sj, nw->u, nw->nzval);
+}
+
+// What precedes each linear solve: the PseudoTransient shift (its SER update once per step, on the first attempt) and the
+// Eisenstat-Walker forcing (every attempt)
+static int32_t pre_step(b200_newton* nw, bool first_attempt, bool fresh) {
+  const b200_newton_opts& o = nw->o;
+  if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT && first_attempt) {
+    // SER (pseudo_transient.jl:157-170): alpha^-1 *= ||f_n|| / ||f_{n-1}||  (2-norm); A = J + alpha^-1 I
+    double rn;
+    B200_TRY(h_nrm2(nw, nw->fu, &rn));
+    nw->alpha_inv *= rn / nw->pt_res_norm;
+    nw->pt_res_norm = rn;
+    nw->op.shift = nw->alpha_inv;
+  }
+  if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT && o.linsolve == B200_LINSOLVE_DENSE_LU && fresh)
+    B200_TRY(b200i_diag_shift(nw->ctx, nw->n, nw->Jdense, nw->n, nw->alpha_inv));  // dampen_jacobian!!: J[i,i] += alpha^-1
+  if (o.forcing == B200_FORCING_EW2 && krylov_linsolve(o)) {  // pre_step_forcing!   eisenstat_walker.jl:42-80
+    if (nw->nsteps == 0) {
+      nw->eta = o.ew_eta0;
+      B200_TRY(h_nrm2(nw, nw->fu, &nw->rnorm));
+      nw->rnorm_prev = nw->rnorm;
+    } else {
+      const double eta_prev = nw->eta;
+      nw->eta = o.ew_gamma * pow(nw->rnorm / nw->rnorm_prev, o.ew_alpha);
+      if (o.ew_safeguard) {
+        const double sg = o.ew_gamma * pow(eta_prev, o.ew_alpha);
+        if (sg > o.ew_safeguard_threshold && sg > nw->eta) nw->eta = sg;
+      }
+      nw->eta = std::min(std::max(nw->eta, 0.0), o.ew_eta_max);
+    }
+    B200_TRY(b200_gmres_set_tolerances(nw->gm, -1.0, nw->eta));  // LinearSolve.update_tolerances!(lincache; reltol = eta)
+  }
+  return B200_OK;
+}
+
+// J xlin = fu (newton.jl:97-141) by the sparse band LU, the dense LU (with its QR rescue) or GMRES; *ok = false is a
+// LinearSolve failure.  *gs holds the GMRES statistics (zero for the direct solvers).
+static int32_t linear_solve(b200_newton* nw, bool fresh, bool* ok, b200_gmres_stats* gs) {
   b200_ctx* ctx = nw->ctx;
   const int64_t n = nw->n;
   const b200_newton_opts& o = nw->o;
-  const double Bv = 8.0 * (double)n;
-  const bool tr_on = o.globalization == B200_GLOBALIZATION_TRUST_REGION;
-  const bool krylov = o.linsolve == B200_LINSOLVE_GMRES || o.linsolve == B200_LINSOLVE_SPARSE_GMRES;
-  const int sch = o.tr_scheme;  // per-scheme defaults  trust_region.jl:348-381
-  const double step_thr = o.tr_step_threshold > 0 ? o.tr_step_threshold : (sch == B200_TR_HEI ? 0.0 : sch == B200_TR_YUAN ? 1.0 / 1000 : sch == B200_TR_BASTIN ? 1.0 / 20 : 1.0 / 10000);
-  const double shrink_thr = o.tr_shrink_threshold > 0 ? o.tr_shrink_threshold : (sch == B200_TR_HEI ? 0.0 : (sch == B200_TR_NLSOLVE || sch == B200_TR_BASTIN) ? 1.0 / 20 : 0.25);
-  const double expand_thr = o.tr_expand_threshold > 0 ? o.tr_expand_threshold : ((sch == B200_TR_NLSOLVE || sch == B200_TR_BASTIN) ? 0.9 : sch == B200_TR_HEI ? 0.0 : 0.75);
-  const double shrink_fac = o.tr_shrink_factor > 0 ? o.tr_shrink_factor : (sch == B200_TR_NLSOLVE ? 0.5 : sch == B200_TR_HEI ? 0.0 : sch == B200_TR_BASTIN ? 1.0 / 20 : 0.25);
-  const double expand_fac = o.tr_expand_factor > 0 ? o.tr_expand_factor : 2.0;
-  const int max_shrink = o.max_shrink_times > 0 ? o.max_shrink_times : 32;
-
-  for (int attempt = 0; attempt < 2; ++attempt) {
-    int new_jacobian;
-    if (nw->make_new_jacobian) {  // J = cache.jac_cache(u)   solve.jl:338-344
-      new_jacobian = 1;
-      if (o.linsolve == B200_LINSOLVE_DENSE_LU) {
-        nw->res.njacs += 1;
-        B200_TRY(b200_dense_jac_fill(nw->prob, nw->u, nw->Jdense, n));  // written straight into the LU workspace (K10: no copyto!)
-        nw->have_factor = 0;
-      } else if (o.linsolve == B200_LINSOLVE_SPARSE_GMRES || o.linsolve == B200_LINSOLVE_SPARSE_LU) {
-        nw->res.njacs += 1;
-        B200_TRY(b200_sparse_jac_fill(nw->sj, nw->u, nw->nzval));
-        nw->have_factor = 0;
+  *ok = true;
+  memset(gs, 0, sizeof(*gs));
+  nw->res.nsolve += 1;
+  if (o.linsolve == B200_LINSOLVE_SPARSE_LU) {
+    if (!nw->have_factor) {
+      nw->res.nfactors += 1;
+      int32_t info = 0;
+      if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT) return ctx->fail(B200_ERR_UNSUPPORTED, "PseudoTransient with the sparse direct solver is not offered (use dense LU or GMRES)", __FILE__, __LINE__);
+      B200_TRY(b200_sparse_lu_factor(nw->slu, nw->nzval, &info));
+      nw->have_factor = 1;
+      if (info != 0) *ok = false;
+    }
+    if (*ok) B200_TRY(b200_sparse_lu_solve(nw->slu, nw->fu, nw->xlin));
+  } else if (!krylov_linsolve(o)) {
+    if (!nw->have_factor) {  // update_A! for a factorisation on a fresh A (…LinearSolveExt.jl:81-86)
+      nw->res.nfactors += 1;
+      int32_t info = 0;
+      B200_TRY(b200_getrf(ctx, n, nw->Jdense, n, nw->ipiv, &info));
+      nw->have_factor = 1;
+      if (info != 0) *ok = false;
+    }
+    CUDA_TRY(ctx, cudaMemcpyAsync(nw->xlin, nw->fu, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (*ok) B200_TRY(b200_getrs(ctx, n, 1, nw->Jdense, n, nw->ipiv, nw->xlin, n));
+    else if (n <= 4096) {
+      // singular LU: LinearSolve's default dense solver falls back to a column-pivoted QR (linear_solve.jl:48-55).  The
+      // factorisation destroyed J: refill it, solve in the least-squares sense (basic solution of the numerical-rank system).
+      B200_TRY(b200_dense_jac_fill(nw->prob, nw->u, nw->Jdense, n));
+      if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT) B200_TRY(b200i_diag_shift(ctx, n, nw->Jdense, n, nw->alpha_inv));
+      if (!nw->qr_work) {
+        B200_TRY(dev_alloc(nw, &nw->qr_work, (size_t)(3 * n + 2), "QR rescue of a singular LU: the workspace does not fit in device memory"));
+        B200_TRY(dev_alloc(nw, &nw->qr_jpvt, (size_t)(n + 2), "QR rescue of a singular LU: the workspace does not fit in device memory"));
       }
-    } else {
-      new_jacobian = 0;
+      CUDA_TRY(ctx, cudaMemcpyAsync(nw->qr_work + 2 * n, nw->fu, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+      int32_t rank = 0;
+      B200_TRY(b200i_qrcp_solve(ctx, n, nw->Jdense, n, nw->qr_work + 2 * n, nw->xlin, nw->qr_work, nw->qr_jpvt, &rank));
+      nw->have_factor = 0;  // Jdense now holds the QR factors: the next step refactorises whatever happens
+      *ok = rank > 0;
     }
-    if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT && attempt == 0) {
-      // SER (pseudo_transient.jl:157-170): alpha^-1 *= ||f_n|| / ||f_{n-1}||  (2-norm); A = J + alpha^-1 I
-      double rn;
-      B200_TRY(h_nrm2(nw, nw->fu, &rn));
-      nw->alpha_inv *= rn / nw->pt_res_norm;
-      nw->pt_res_norm = rn;
-      nw->op.shift = nw->alpha_inv;
-    }
-    if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT && o.linsolve == B200_LINSOLVE_DENSE_LU && new_jacobian)
-      B200_TRY(b200i_diag_shift(ctx, n, nw->Jdense, n, nw->alpha_inv));  // dampen_jacobian!!: J[i,i] += alpha^-1
-    if (o.forcing == B200_FORCING_EW2 && krylov) {  // pre_step_forcing!   eisenstat_walker.jl:42-80
-      if (nw->nsteps == 0) {
-        nw->eta = o.ew_eta0;
-        B200_TRY(h_nrm2(nw, nw->fu, &nw->rnorm));
-        nw->rnorm_prev = nw->rnorm;
+  } else {
+    // `linu` aliases the du buffer: it is the initial guess only when warm_start is requested
+    if (o.gmres.warm_start) CUDA_TRY(ctx, cudaMemcpyAsync(nw->xlin, nw->du, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (o.precond != B200_PRECOND_NONE) {  // precs(A, p): rebuilt from the current iterate, like update_A! does for Pl / Pr
+      memset(&nw->prec, 0, sizeof(nw->prec));
+      nw->prec.ctx = ctx; nw->prec.n = n; nw->prec.prob = nw->prob; nw->prec.u = nw->u;
+      if (nw->mg) {
+        nw->prec.kind = LINOP_MULTIGRID; nw->prec.mg = nw->mg;
+        if (fresh) B200_TRY(b200i_mg_setup(nw->mg, nw->u));  // coarse operators follow the linearisation point
       } else {
-        const double eta_prev = nw->eta;
-        nw->eta = o.ew_gamma * pow(nw->rnorm / nw->rnorm_prev, o.ew_alpha);
-        if (o.ew_safeguard) {
-          const double sg = o.ew_gamma * pow(eta_prev, o.ew_alpha);
-          if (sg > o.ew_safeguard_threshold && sg > nw->eta) nw->eta = sg;
-        }
-        nw->eta = std::min(std::max(nw->eta, 0.0), o.ew_eta_max);
+        nw->prec.kind = LINOP_BLOCK_JACOBI;
       }
-      B200_TRY(b200_gmres_set_tolerances(nw->gm, -1.0, nw->eta));  // LinearSolve.update_tolerances!(lincache; reltol = eta)
+      const bool left = o.precond == B200_PRECOND_BLOCK_JACOBI_LEFT || o.precond == B200_PRECOND_MULTIGRID_LEFT;
+      B200_TRY(b200_gmres_set_precond(nw->gm, left ? &nw->prec : nullptr, left ? nullptr : &nw->prec));
     }
-    // ---- descent: J x = fu ; du = -x   (newton.jl:97-141)
-    int lin_success = 1;
-    b200_gmres_stats gs;
-    memset(&gs, 0, sizeof(gs));
-    nw->res.nsolve += 1;
-    if (o.linsolve == B200_LINSOLVE_SPARSE_LU) {
-      if (!nw->have_factor) {
-        nw->res.nfactors += 1;
-        int32_t info = 0;
-        if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT) return ctx->fail(B200_ERR_UNSUPPORTED, "PseudoTransient with the sparse direct solver is not offered (use dense LU or GMRES)", __FILE__, __LINE__);
-        B200_TRY(b200_sparse_lu_factor(nw->slu, nw->nzval, &info));
-        nw->have_factor = 1;
-        if (info != 0) lin_success = 0;
-      }
-      if (lin_success) B200_TRY(b200_sparse_lu_solve(nw->slu, nw->fu, nw->xlin));
-    } else if (!krylov) {
-      if (!nw->have_factor) {  // update_A! for a factorisation on a fresh A (…LinearSolveExt.jl:81-86)
-        nw->res.nfactors += 1;
-        int32_t info = 0;
-        B200_TRY(b200_getrf(ctx, n, nw->Jdense, n, nw->ipiv, &info));
-        nw->have_factor = 1;
-        if (info != 0) lin_success = 0;
-      }
-      CUDA_TRY(ctx, cudaMemcpyAsync(nw->xlin, nw->fu, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-      if (lin_success) B200_TRY(b200_getrs(ctx, n, 1, nw->Jdense, n, nw->ipiv, nw->xlin, n));
-      else if (n <= 4096) {
-        // singular LU: LinearSolve's default dense solver falls back to a column-pivoted QR (linear_solve.jl:48-55).  The
-        // factorisation destroyed J: refill it, solve in the least-squares sense (basic solution of the numerical-rank system).
-        B200_TRY(b200_dense_jac_fill(nw->prob, nw->u, nw->Jdense, n));
-        if (o.descent == B200_DESCENT_PSEUDO_TRANSIENT) B200_TRY(b200i_diag_shift(ctx, n, nw->Jdense, n, nw->alpha_inv));
-        if (!nw->qr_work) {
-          CUDA_TRY(ctx, cudaMalloc(&nw->qr_work, sizeof(double) * (3 * n + 2)));
-          CUDA_TRY(ctx, cudaMalloc(&nw->qr_jpvt, sizeof(int32_t) * (n + 2)));
-        }
-        CUDA_TRY(ctx, cudaMemcpyAsync(nw->qr_work + 2 * n, nw->fu, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-        int32_t rank = 0;
-        B200_TRY(b200i_qrcp_solve(ctx, n, nw->Jdense, n, nw->qr_work + 2 * n, nw->xlin, nw->qr_work, nw->qr_jpvt, &rank));
-        nw->have_factor = 0;  // Jdense now holds the QR factors: the next step refactorises whatever happens
-        lin_success = rank > 0 ? 1 : 0;
-      }
-    } else {
-      // `linu` aliases the du buffer: it is the initial guess only when warm_start is requested
-      if (o.gmres.warm_start) CUDA_TRY(ctx, cudaMemcpyAsync(nw->xlin, nw->du, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-      if (o.precond != B200_PRECOND_NONE) {  // precs(A, p): rebuilt from the current iterate, like update_A! does for Pl / Pr
-        memset(&nw->prec, 0, sizeof(nw->prec));
-        nw->prec.ctx = ctx; nw->prec.n = n; nw->prec.prob = nw->prob; nw->prec.u = nw->u;
-        if (nw->mg) {
-          nw->prec.kind = LINOP_MULTIGRID; nw->prec.mg = nw->mg;
-          if (new_jacobian) B200_TRY(b200i_mg_setup(nw->mg, nw->u));  // coarse operators follow the linearisation point
-        } else {
-          nw->prec.kind = LINOP_BLOCK_JACOBI;
-        }
-        const bool left = o.precond == B200_PRECOND_BLOCK_JACOBI_LEFT || o.precond == B200_PRECOND_MULTIGRID_LEFT;
-        B200_TRY(b200_gmres_set_precond(nw->gm, left ? &nw->prec : nullptr, left ? nullptr : &nw->prec));
-      }
-      B200_TRY(b200_gmres_solve(nw->gm, &nw->op, nw->fu, nw->xlin, &gs));
-      nw->res.njvp += gs.nmatvec;
-      nw->bytes += gs.bytes;
-      if (gs.status == B200_LS_NONFINITE || gs.status == B200_LS_OUT_OF_MEMORY) lin_success = 0;  // LinearSolve retcode Failure
-    }
-    if (!lin_success) {  // solve.jl:367-382
-      if (new_jacobian) { nw->retcode = B200_RC_INTERNAL_LINSOLVE_FAILED; nw->force_stop = 1; return B200_OK; }
-      nw->make_new_jacobian = 1;
-      continue;  // retry once with a fresh Jacobian
-    }
-    // du = -x   (@. du *= -1, newton.jl:138)
-    B200_TRY(b200_axpby(ctx, n, -1.0, nw->xlin, 0.0, nw->du));
-
-    double dJJd = NAN;
-    if (tr_on) {  // Dogleg   dogleg.jl:86-151
-      double nrm_newton;
-      B200_TRY(h_nrm2(nw, nw->du, &nrm_newton));
-      if (!(nrm_newton <= nw->trust_region)) {
-        B200_TRY(b200_vjp(nw->prob, nw->u, nw->fu, nw->du_c));  // du_c = -J' fu  (steepest.jl:60-80)
-        B200_TRY(b200_scal(ctx, n, -1.0, nw->du_c));
-        double l_grad, quad;
-        B200_TRY(h_nrm2(nw, nw->du_c, &l_grad));
-        B200_TRY(b200_jvp(nw->prob, nw->u, nw->du_c, nw->Jdu));
-        B200_TRY(h_dot(nw, nw->Jdu, nw->Jdu, &quad));
-        const double d_cauchy = (l_grad * l_grad * l_grad) / quad;
-        if (d_cauchy >= nw->trust_region) {
-          const double lam = nw->trust_region / l_grad;
-          B200_TRY(b200_axpby(ctx, n, lam, nw->du_c, 0.0, nw->du));
-          dJJd = lam * lam * quad;
-        } else {
-          B200_TRY(b200_axpby(ctx, n, d_cauchy / l_grad, nw->du_c, 0.0, nw->c1));  // c1 = (d_cauchy/l_grad) du_c
-          B200_TRY(b200_copy(ctx, n, nw->du, nw->c2));
-          B200_TRY(b200_axpy(ctx, n, -1.0, nw->c1, nw->c2));                         // c2 = du_newton - c1
-          B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->c2, nw->c2, RED_DOT, ctx->d_scalars));
-          B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->c1, nw->c2, RED_DOT, ctx->d_scalars + 1));
-          B200_TRY(b200i_fetch_scalars(ctx, 2));
-          const double a = ctx->h_scalars[0], b2 = ctx->h_scalars[1];
-          const double b = 2.0 * b2, c = d_cauchy * d_cauchy - nw->trust_region * nw->trust_region;
-          const double aux = std::max(0.0, b * b - 4.0 * a * c);
-          const double tau = (-b + sqrt(aux)) / (2.0 * a);
-          B200_TRY(b200_copy(ctx, n, nw->c1, nw->du));
-          B200_TRY(b200_axpy(ctx, n, tau, nw->c2, nw->du));
-        }
-      }
-    }
-    if (o.forcing == B200_FORCING_EW2 && krylov) {  // post_step_forcing!  eisenstat_walker.jl:83-87 (fu is still the old residual)
-      nw->rnorm_prev = nw->rnorm;
-      B200_TRY(h_nrm2(nw, nw->fu, &nw->rnorm));
-    }
-    nw->make_new_jacobian = 1;
-    int accepted = 1;
-    double objective, du_norm;
-    double ls_alpha = 1.0;
-    if (o.globalization == B200_GLOBALIZATION_LINESEARCH) {
-      // solve.jl:392-408 with LineSearch.jl BackTracking (cubic interpolation; external package restated, see oracle.c):
-      // phi(a) = ||f(u + a du)||^2 / 2, phi'(0) = <fu, J du> by one JVP; every trial is one axpby + one residual + one norm.
-      const double c1 = o.ls_c1 > 0 ? o.ls_c1 : 1e-4, rho_hi = o.ls_rho_hi > 0 ? o.ls_rho_hi : 0.5, rho_lo = o.ls_rho_lo > 0 ? o.ls_rho_lo : 0.1;
-      const int ls_max = o.ls_maxiters > 0 ? o.ls_maxiters : 1000;
-      double nf0, dphi0;
-      B200_TRY(h_nrm2(nw, nw->fu, &nf0));
-      const double phi0 = 0.5 * nf0 * nf0;
-      B200_TRY(b200_jvp(nw->prob, nw->u, nw->du, nw->Jdu));
-      B200_TRY(h_dot(nw, nw->fu, nw->Jdu, &dphi0));
-      auto phi = [&](double alpha, double* out) -> int32_t {
-        B200_TRY(b200_copy(ctx, n, nw->u, nw->u_trial));
-        B200_TRY(b200_axpy(ctx, n, alpha, nw->du, nw->u_trial));
-        B200_TRY(b200_residual(nw->prob, nw->u_trial, nw->fu_trial));
-        nw->res.nf += 1;
-        double t;
-        B200_TRY(h_nrm2(nw, nw->fu_trial, &t));
-        *out = 0.5 * t * t;
-        return B200_OK;
-      };
-      double a1 = 1.0, a2 = 1.0, phx0 = phi0, phx1;
-      B200_TRY(phi(a1, &phx1));
-      int itf = 0;
-      while (!std::isfinite(phx1) && itf < 50) { ++itf; a1 = a2; a2 = a1 / 2.0; B200_TRY(phi(a2, &phx1)); }
-      int it = 0, ls_failed = 0;
-      while (phx1 > phi0 + c1 * a2 * dphi0) {
-        if (++it > ls_max) { ls_failed = 1; break; }
-        double at;
-        if (it == 1) at = -(dphi0 * a2 * a2) / (2.0 * (phx1 - phi0 - dphi0 * a2));
-        else {
-          const double div = 1.0 / (a1 * a1 * a2 * a2 * (a2 - a1));
-          const double ca = (a1 * a1 * (phx1 - phi0 - dphi0 * a2) - a2 * a2 * (phx0 - phi0 - dphi0 * a1)) * div;
-          const double cb = (-a1 * a1 * a1 * (phx1 - phi0 - dphi0 * a2) + a2 * a2 * a2 * (phx0 - phi0 - dphi0 * a1)) * div;
-          if (fabs(ca) <= 1e-14 * fabs(cb) || ca == 0.0) at = dphi0 / (2.0 * cb);
-          else { const double dd = std::max(cb * cb - 3.0 * ca * dphi0, 0.0); at = (-cb + sqrt(dd)) / (3.0 * ca); }
-        }
-        a1 = a2;
-        at = std::min(at, a2 * rho_hi);
-        a2 = std::max(at, a2 * rho_lo);
-        phx0 = phx1;
-        B200_TRY(phi(a2, &phx1));
-      }
-      if (ls_failed) { nw->retcode = B200_RC_INTERNAL_LINESEARCH_FAILED; nw->force_stop = 1; }
-      ls_alpha = a2;
-      CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
-      B200_TRY(b200i_axpy_norm(ctx, n, a2, nw->du, nw->u, ctx->d_scalars + 1));   // @bb axpy!(alpha, du, u)   solve.jl:403
-      B200_TRY(b200i_residual_norm(nw->prob, nw->u, nw->fu, ctx->d_scalars));     // evaluate_f!               solve.jl:407
-      nw->res.nf += 1;
-      B200_TRY(b200i_fetch_scalars(ctx, 2));
-      objective = ctx->h_scalars[0];
-      du_norm = sqrt(ctx->h_scalars[1]);
-    } else if (!tr_on) {  // solve.jl:436-445 : u += du ; fu = f(u) ; with ||du||^2 and ||fu||_inf produced by the kernels' epilogues
-      CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
-      B200_TRY(b200i_axpy_norm(ctx, n, 1.0, nw->du, nw->u, ctx->d_scalars + 1));
-      B200_TRY(b200i_residual_norm(nw->prob, nw->u, nw->fu, ctx->d_scalars));
-      nw->res.nf += 1;
-      B200_TRY(b200i_fetch_scalars(ctx, 2));
-      objective = ctx->h_scalars[0];
-      du_norm = sqrt(ctx->h_scalars[1]);
-      nw->bytes += 5.0 * Bv;
-    } else {  // GenericTrustRegionScheme solve!   trust_region.jl:396-430, 511-513
-      B200_TRY(b200_copy(ctx, n, nw->u, nw->u_trial));
-      B200_TRY(b200_axpy(ctx, n, 1.0, nw->du, nw->u_trial));
-      CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
-      B200_TRY(b200i_residual_norm(nw->prob, nw->u_trial, nw->fu_trial, ctx->d_scalars));
-      nw->res.nf += 1;
-      // the six scalars of the acceptance test are independent: reduced on the device one after the other, fetched ONCE
-      // (round 1 synchronised the host after each of them; VERDICT r1 weak #11)
-      const bool need_dJJd = dJJd != dJJd;
-      if (need_dJJd) {
-        B200_TRY(b200_jvp(nw->prob, nw->u, nw->du, nw->Jdu));
-        B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->Jdu, nw->Jdu, RED_DOT, ctx->d_scalars + 1));
-      }
-      B200_TRY(b200_vjp(nw->prob, nw->u, nw->fu, nw->JTfu));
-      B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->fu_trial, nullptr, RED_SUMSQ, ctx->d_scalars + 2));
-      B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->fu, nullptr, RED_SUMSQ, ctx->d_scalars + 3));
-      B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->du, nw->JTfu, RED_DOT, ctx->d_scalars + 4));
-      B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->du, nullptr, RED_SUMSQ, ctx->d_scalars + 5));
-      B200_TRY(b200i_fetch_scalars(ctx, 6));
-      const double trial_inf = ctx->h_scalars[0];
-      if (need_dJJd) dJJd = ctx->h_scalars[1];
-      const double nt = sqrt(ctx->h_scalars[2]), nc = sqrt(ctx->h_scalars[3]), dg = ctx->h_scalars[4];
-      const double num = (nt * nt - nc * nc) / 2.0;
-      const double denom = dg + dJJd / 2.0;
-      const double rho = num / denom;
-      accepted = rho > step_thr;
-      const double dun = sqrt(ctx->h_scalars[5]);  // internalnorm(du)
-      double& tr = nw->trust_region;
-      if (sch == B200_TR_SIMPLE) {  // trust_region.jl:431-440
-        if (rho < shrink_thr) { tr *= shrink_fac; nw->shrink_counter += 1; }
-        else { nw->shrink_counter = 0; if (rho > expand_thr && rho > step_thr) tr = expand_fac * tr; }
-      } else if (sch == B200_TR_NLSOLVE) {  // :441-455
-        if (rho < shrink_thr) { tr *= shrink_fac; nw->shrink_counter += 1; }
-        else {
-          nw->shrink_counter = 0;
-          if (rho >= expand_thr) tr = expand_fac * dun;
-          else if (rho >= nw->tp1) tr = std::max(tr, expand_fac * dun);
-        }
-      } else if (sch == B200_TR_NOCEDAL_WRIGHT) {  // :456-466
-        if (rho < shrink_thr) { tr = shrink_fac * dun; nw->shrink_counter += 1; }
-        else { nw->shrink_counter = 0; if (rho > expand_thr && fabs(dun - tr) < 1.0e-6 * tr) tr = expand_fac * tr; }
-      } else if (sch == B200_TR_HEI) {  // :467-476, rfunc_adaptive_trust_region :383-391
-        const double M = nw->tp1, g1 = nw->tp3, g2 = nw->tp4, beta = nw->tp2;
-        const double rf = (rho >= shrink_thr) ? (2.0 * (M - 1.0 - g2) * atan(rho - shrink_thr) + (1.0 + g2)) / M_PI
-                                              : (1.0 - g1 - beta) * (exp(rho - shrink_thr) + beta / (1.0 - g1 - beta));
-        const double tr_new = rf * dun;
-        if (tr_new < tr) nw->shrink_counter += 1; else nw->shrink_counter = 0;
-        tr = tr_new;
-      } else if (sch == B200_TR_YUAN) {  // :477-490
-        if (rho < shrink_thr) { nw->tp1 = nw->tp2 * nw->tp1; nw->shrink_counter += 1; }
-        else { if (rho >= expand_thr && 2.0 * dun > tr) nw->tp1 = nw->tp3 * nw->tp1; nw->shrink_counter = 0; }
-        double g;
-        B200_TRY(b200_vjp(nw->prob, nw->u_trial, nw->fu_trial, nw->JTfu));
-        B200_TRY(h_nrm2(nw, nw->JTfu, &g));
-        tr = nw->tp1 * g;
-      } else if (sch == B200_TR_FAN) {  // :491-499
-        if (rho < shrink_thr) { nw->tp1 *= nw->tp2; nw->shrink_counter += 1; }
-        else { nw->shrink_counter = 0; if (rho > expand_thr) nw->tp1 = std::min(nw->tp1 * nw->tp3, nw->tp4); }
-        tr = nw->tp1 * pow(nt, 0.99);
-      } else if (sch == B200_TR_BASTIN) {  // :500-520, retrospective ratio at the trial point with the step just taken
-        if (rho > step_thr) {
-          double d1, d2;
-          B200_TRY(b200_jvp(nw->prob, nw->u_trial, nw->du, nw->Jdu));
-          B200_TRY(b200_vjp(nw->prob, nw->u_trial, nw->fu_trial, nw->JTfu));
-          B200_TRY(h_dot(nw, nw->JTfu, nw->JTfu, &d1));
-          B200_TRY(b200_vjp(nw->prob, nw->u_trial, nw->Jdu, nw->JTfu));
-          B200_TRY(h_dot(nw, nw->JTfu, nw->JTfu, &d2));
-          const double rho_retro = num / (d1 + d2 / 2.0);
-          if (rho_retro >= expand_thr) tr = nw->tp1 * dun;
-          nw->shrink_counter = 0;
-        } else { tr *= nw->tp2; nw->shrink_counter += 1; }
-      }
-      nw->trust_region = std::min(nw->trust_region, nw->max_tr);
-      if (accepted) {
-        du_norm = dun;
-        std::swap(nw->u, nw->u_trial);      // copyto!(cache.u, u_new) as a pointer swap
-        std::swap(nw->fu, nw->fu_trial);
-        nw->op.u = nw->u;
-        objective = trial_inf;
-      } else {
-        nw->make_new_jacobian = 0;
-        objective = nw->fnorm_inf;
-        du_norm = 0.0;
-      }
-      if (nw->shrink_counter > max_shrink) { nw->retcode = B200_RC_SHRINK_THRESHOLD_EXCEEDED; nw->force_stop = 1; }
-    }
-    nw->fnorm_inf = objective;
-    bool new_best = false;
-    TermQuant tq;
-    B200_TRY(term_quantities(nw, nw->fu, nw->u, objective, &tq));
-    if (term_check(nw, tq, du_norm, &new_best)) { nw->retcode = nw->tc.retcode; nw->force_stop = 1; }  // check_and_update!
-    if (new_best && nw->best_u) CUDA_TRY(ctx, cudaMemcpyAsync(nw->best_u, nw->u, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
-    if (o.store_trace) {
-      b200_trace_rec t;
-      t.iter = nw->nsteps + 1; t.lin_iters = gs.iters; t.lin_status = gs.status; t.accepted = accepted;
-      t.fnorm_inf = objective; t.step_norm2 = du_norm; t.lin_rnorm = gs.rnorm; t.trust_radius = (o.globalization == B200_GLOBALIZATION_LINESEARCH) ? ls_alpha : (o.descent == B200_DESCENT_PSEUDO_TRANSIENT) ? 1.0 / nw->alpha_inv : nw->trust_region;
-      nw->trace.push_back(t);
-    }
-    // copyto!(u_cache, u) (solve.jl:460) is only ever read back as `uprev` for the stall norm, which the update kernel
-    // already produced; the copy is skipped.
-    return B200_OK;
+    B200_TRY(b200_gmres_solve(nw->gm, &nw->op, nw->fu, nw->xlin, gs));
+    nw->res.njvp += gs->nmatvec;
+    nw->bytes += gs->bytes;
+    if (gs->status == B200_LS_NONFINITE || gs->status == B200_LS_OUT_OF_MEMORY) *ok = false;  // LinearSolve retcode Failure
   }
   return B200_OK;
+}
+
+// Dogleg (dogleg.jl:86-151): du holds the Newton step on entry and the dogleg step on return.  When the step is the Cauchy
+// direction cut at the radius, ||J du||^2 is already known: *have_dJJd is set and *dJJd holds it.
+static int32_t dogleg(b200_newton* nw, bool* have_dJJd, double* dJJd) {
+  b200_ctx* ctx = nw->ctx;
+  const int64_t n = nw->n;
+  *have_dJJd = false;
+  double nrm_newton;
+  B200_TRY(h_nrm2(nw, nw->du, &nrm_newton));
+  if (nrm_newton <= nw->trust_region) return B200_OK;
+  B200_TRY(b200_vjp(nw->prob, nw->u, nw->fu, nw->du_c));  // du_c = -J' fu  (steepest.jl:60-80)
+  B200_TRY(b200_scal(ctx, n, -1.0, nw->du_c));
+  double l_grad, quad;
+  B200_TRY(h_nrm2(nw, nw->du_c, &l_grad));
+  B200_TRY(b200_jvp(nw->prob, nw->u, nw->du_c, nw->Jdu));
+  B200_TRY(h_dot(nw, nw->Jdu, nw->Jdu, &quad));
+  const double d_cauchy = (l_grad * l_grad * l_grad) / quad;
+  if (d_cauchy >= nw->trust_region) {
+    const double lam = nw->trust_region / l_grad;
+    B200_TRY(b200_axpby(ctx, n, lam, nw->du_c, 0.0, nw->du));
+    *have_dJJd = true;
+    *dJJd = lam * lam * quad;
+    return B200_OK;
+  }
+  B200_TRY(b200_axpby(ctx, n, d_cauchy / l_grad, nw->du_c, 0.0, nw->c1));  // c1 = (d_cauchy/l_grad) du_c
+  B200_TRY(b200_copy(ctx, n, nw->du, nw->c2));
+  B200_TRY(b200_axpy(ctx, n, -1.0, nw->c1, nw->c2));                         // c2 = du_newton - c1
+  B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->c2, nw->c2, RED_DOT, ctx->d_scalars));
+  B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->c1, nw->c2, RED_DOT, ctx->d_scalars + 1));
+  B200_TRY(b200i_fetch_scalars(ctx, 2));
+  const double a = ctx->h_scalars[0], b2 = ctx->h_scalars[1];
+  const double b = 2.0 * b2, c = d_cauchy * d_cauchy - nw->trust_region * nw->trust_region;
+  const double aux = std::max(0.0, b * b - 4.0 * a * c);
+  const double tau = (-b + sqrt(aux)) / (2.0 * a);
+  B200_TRY(b200_copy(ctx, n, nw->c1, nw->du));
+  return b200_axpy(ctx, n, tau, nw->c2, nw->du);
+}
+
+// solve.jl:392-408 with LineSearch.jl BackTracking (cubic interpolation; external package restated, see oracle.c):
+// phi(a) = ||f(u + a du)||^2 / 2, phi'(0) = <fu, J du> by one JVP; every trial is one axpby + one residual + one norm.
+// *alpha is the step length to take; a search that runs out of iterations stops the solve with LINESEARCH_FAILED.
+static int32_t backtracking(b200_newton* nw, double* alpha) {
+  const b200_newton_opts& o = nw->o;
+  const double c1 = o.ls_c1 > 0 ? o.ls_c1 : 1e-4, rho_hi = o.ls_rho_hi > 0 ? o.ls_rho_hi : 0.5, rho_lo = o.ls_rho_lo > 0 ? o.ls_rho_lo : 0.1;
+  const int ls_max = o.ls_maxiters > 0 ? o.ls_maxiters : 1000;
+  double nf0, dphi0;
+  B200_TRY(h_nrm2(nw, nw->fu, &nf0));
+  const double phi0 = 0.5 * nf0 * nf0;
+  B200_TRY(b200_jvp(nw->prob, nw->u, nw->du, nw->Jdu));
+  B200_TRY(h_dot(nw, nw->fu, nw->Jdu, &dphi0));
+  auto phi = [&](double a, double* out) -> int32_t {
+    B200_TRY(trial_point(nw, a, nw->du));
+    B200_TRY(b200_residual(nw->prob, nw->u_trial, nw->fu_trial));
+    nw->res.nf += 1;
+    double t;
+    B200_TRY(h_nrm2(nw, nw->fu_trial, &t));
+    *out = 0.5 * t * t;
+    return B200_OK;
+  };
+  double a1 = 1.0, a2 = 1.0, phx0 = phi0, phx1;
+  B200_TRY(phi(a1, &phx1));
+  int itf = 0;
+  while (!std::isfinite(phx1) && itf < 50) { ++itf; a1 = a2; a2 = a1 / 2.0; B200_TRY(phi(a2, &phx1)); }
+  int it = 0;
+  while (phx1 > phi0 + c1 * a2 * dphi0) {
+    if (++it > ls_max) { nw->retcode = B200_RC_INTERNAL_LINESEARCH_FAILED; nw->force_stop = 1; break; }
+    double at;
+    if (it == 1) at = -(dphi0 * a2 * a2) / (2.0 * (phx1 - phi0 - dphi0 * a2));
+    else {
+      const double div = 1.0 / (a1 * a1 * a2 * a2 * (a2 - a1));
+      const double ca = (a1 * a1 * (phx1 - phi0 - dphi0 * a2) - a2 * a2 * (phx0 - phi0 - dphi0 * a1)) * div;
+      const double cb = (-a1 * a1 * a1 * (phx1 - phi0 - dphi0 * a2) + a2 * a2 * a2 * (phx0 - phi0 - dphi0 * a1)) * div;
+      if (fabs(ca) <= 1e-14 * fabs(cb) || ca == 0.0) at = dphi0 / (2.0 * cb);
+      else { const double dd = std::max(cb * cb - 3.0 * ca * dphi0, 0.0); at = (-cb + sqrt(dd)) / (3.0 * ca); }
+    }
+    a1 = a2;
+    at = std::min(at, a2 * rho_hi);
+    a2 = std::max(at, a2 * rho_lo);
+    phx0 = phx1;
+    B200_TRY(phi(a2, &phx1));
+  }
+  *alpha = a2;
+  return B200_OK;
+}
+
+// GenericTrustRegionScheme solve! (trust_region.jl:396-430, 511-513): the trial point u + du, the ratio rho of actual to
+// predicted decrease, the radius update of the scheme (:431-520), then the step is taken or not.  dJJd = ||J du||^2 when the
+// dogleg already has it.
+static int32_t trust_region_step(b200_newton* nw, bool have_dJJd, double dJJd, int* accepted, double* objective, double* du_norm) {
+  b200_ctx* ctx = nw->ctx;
+  const int64_t n = nw->n;
+  const TrParams& p = nw->trp;
+  B200_TRY(trial_point(nw, 1.0, nw->du));
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 2, ctx->stream));
+  B200_TRY(b200i_residual_norm(nw->prob, nw->u_trial, nw->fu_trial, ctx->d_scalars));
+  nw->res.nf += 1;
+  // the six scalars of the acceptance test are independent: reduced on the device one after the other, fetched ONCE
+  // (round 1 synchronised the host after each of them; VERDICT r1 weak #11)
+  if (!have_dJJd) {
+    B200_TRY(b200_jvp(nw->prob, nw->u, nw->du, nw->Jdu));
+    B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->Jdu, nw->Jdu, RED_DOT, ctx->d_scalars + 1));
+  }
+  B200_TRY(b200_vjp(nw->prob, nw->u, nw->fu, nw->JTfu));
+  B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->fu_trial, nullptr, RED_SUMSQ, ctx->d_scalars + 2));
+  B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->fu, nullptr, RED_SUMSQ, ctx->d_scalars + 3));
+  B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->du, nw->JTfu, RED_DOT, ctx->d_scalars + 4));
+  B200_TRY(b200i_reduce_sum_dev(ctx, n, nw->du, nullptr, RED_SUMSQ, ctx->d_scalars + 5));
+  B200_TRY(b200i_fetch_scalars(ctx, 6));
+  const double trial_inf = ctx->h_scalars[0];
+  if (!have_dJJd) dJJd = ctx->h_scalars[1];
+  const double nt = sqrt(ctx->h_scalars[2]), nc = sqrt(ctx->h_scalars[3]), dg = ctx->h_scalars[4];
+  const double num = (nt * nt - nc * nc) / 2.0;
+  const double denom = dg + dJJd / 2.0;
+  const double rho = num / denom;
+  *accepted = rho > p.step_thr;
+  const double dun = sqrt(ctx->h_scalars[5]);  // internalnorm(du)
+  const int sch = nw->o.tr_scheme;
+  double& tr = nw->trust_region;
+  if (sch == B200_TR_SIMPLE) {  // trust_region.jl:431-440
+    if (rho < p.shrink_thr) { tr *= p.shrink_fac; nw->shrink_counter += 1; }
+    else { nw->shrink_counter = 0; if (rho > p.expand_thr && rho > p.step_thr) tr = p.expand_fac * tr; }
+  } else if (sch == B200_TR_NLSOLVE) {  // :441-455
+    if (rho < p.shrink_thr) { tr *= p.shrink_fac; nw->shrink_counter += 1; }
+    else {
+      nw->shrink_counter = 0;
+      if (rho >= p.expand_thr) tr = p.expand_fac * dun;
+      else if (rho >= nw->tp1) tr = std::max(tr, p.expand_fac * dun);
+    }
+  } else if (sch == B200_TR_NOCEDAL_WRIGHT) {  // :456-466
+    if (rho < p.shrink_thr) { tr = p.shrink_fac * dun; nw->shrink_counter += 1; }
+    else { nw->shrink_counter = 0; if (rho > p.expand_thr && fabs(dun - tr) < 1.0e-6 * tr) tr = p.expand_fac * tr; }
+  } else if (sch == B200_TR_HEI) {  // :467-476, rfunc_adaptive_trust_region :383-391
+    const double M = nw->tp1, g1 = nw->tp3, g2 = nw->tp4, beta = nw->tp2;
+    const double rf = (rho >= p.shrink_thr) ? (2.0 * (M - 1.0 - g2) * atan(rho - p.shrink_thr) + (1.0 + g2)) / M_PI
+                                            : (1.0 - g1 - beta) * (exp(rho - p.shrink_thr) + beta / (1.0 - g1 - beta));
+    const double tr_new = rf * dun;
+    if (tr_new < tr) nw->shrink_counter += 1; else nw->shrink_counter = 0;
+    tr = tr_new;
+  } else if (sch == B200_TR_YUAN) {  // :477-490
+    if (rho < p.shrink_thr) { nw->tp1 = nw->tp2 * nw->tp1; nw->shrink_counter += 1; }
+    else { if (rho >= p.expand_thr && 2.0 * dun > tr) nw->tp1 = nw->tp3 * nw->tp1; nw->shrink_counter = 0; }
+    double g;
+    B200_TRY(b200_vjp(nw->prob, nw->u_trial, nw->fu_trial, nw->JTfu));
+    B200_TRY(h_nrm2(nw, nw->JTfu, &g));
+    tr = nw->tp1 * g;
+  } else if (sch == B200_TR_FAN) {  // :491-499
+    if (rho < p.shrink_thr) { nw->tp1 *= nw->tp2; nw->shrink_counter += 1; }
+    else { nw->shrink_counter = 0; if (rho > p.expand_thr) nw->tp1 = std::min(nw->tp1 * nw->tp3, nw->tp4); }
+    tr = nw->tp1 * pow(nt, 0.99);
+  } else if (sch == B200_TR_BASTIN) {  // :500-520, retrospective ratio at the trial point with the step just taken
+    if (rho > p.step_thr) {
+      double d1, d2;
+      B200_TRY(b200_jvp(nw->prob, nw->u_trial, nw->du, nw->Jdu));
+      B200_TRY(b200_vjp(nw->prob, nw->u_trial, nw->fu_trial, nw->JTfu));
+      B200_TRY(h_dot(nw, nw->JTfu, nw->JTfu, &d1));
+      B200_TRY(b200_vjp(nw->prob, nw->u_trial, nw->Jdu, nw->JTfu));
+      B200_TRY(h_dot(nw, nw->JTfu, nw->JTfu, &d2));
+      const double rho_retro = num / (d1 + d2 / 2.0);
+      if (rho_retro >= p.expand_thr) tr = nw->tp1 * dun;
+      nw->shrink_counter = 0;
+    } else { tr *= nw->tp2; nw->shrink_counter += 1; }
+  }
+  tr = std::min(tr, nw->max_tr);
+  if (*accepted) {
+    accept_trial(nw);
+    *objective = trial_inf;
+    *du_norm = dun;
+  } else {
+    nw->make_new_jacobian = 0;
+    *objective = nw->fnorm_inf;
+    *du_norm = 0.0;
+  }
+  if (nw->shrink_counter > p.max_shrink) { nw->retcode = B200_RC_SHRINK_THRESHOLD_EXCEEDED; nw->force_stop = 1; }
+  return B200_OK;
+}
+
+// step! (solve.jl:325-465): refresh J, solve, retry once with a fresh Jacobian, descend, globalise, end the step
+static int32_t newton_step_inner(b200_newton* nw) {
+  if (nw->o.descent == B200_DESCENT_LEVENBERG_MARQUARDT) return lm_step(nw);
+  if (nw->o.descent == B200_DESCENT_BROYDEN) return broyden_step(nw);
+  const b200_newton_opts& o = nw->o;
+  bool fresh, ok;
+  b200_gmres_stats gs;
+  auto attempt = [&](bool first) -> int32_t {
+    B200_TRY(refresh_jacobian(nw, &fresh));
+    B200_TRY(pre_step(nw, first, fresh));
+    return linear_solve(nw, fresh, &ok, &gs);
+  };
+  B200_TRY(attempt(true));
+  if (!ok && !fresh) {  // solve.jl:367-382
+    nw->make_new_jacobian = 1;
+    B200_TRY(attempt(false));
+  }
+  if (!ok) { nw->retcode = B200_RC_INTERNAL_LINSOLVE_FAILED; nw->force_stop = 1; return B200_OK; }
+  B200_TRY(b200_axpby(nw->ctx, nw->n, -1.0, nw->xlin, 0.0, nw->du));  // du = -x   (@. du *= -1, newton.jl:138)
+  const bool tr_on = o.globalization == B200_GLOBALIZATION_TRUST_REGION;
+  bool have_dJJd = false;
+  double dJJd = 0.0;
+  if (tr_on) B200_TRY(dogleg(nw, &have_dJJd, &dJJd));
+  if (o.forcing == B200_FORCING_EW2 && krylov_linsolve(o)) {  // post_step_forcing!  eisenstat_walker.jl:83-87 (fu is still the old residual)
+    nw->rnorm_prev = nw->rnorm;
+    B200_TRY(h_nrm2(nw, nw->fu, &nw->rnorm));
+  }
+  nw->make_new_jacobian = 1;
+  const bool ls_on = o.globalization == B200_GLOBALIZATION_LINESEARCH;
+  int accepted = 1;
+  double objective, du_norm, alpha = 1.0;
+  if (ls_on) {
+    B200_TRY(backtracking(nw, &alpha));
+    B200_TRY(update_u(nw, alpha, &objective, &du_norm));  // @bb axpy!(alpha, du, u) ; evaluate_f!   solve.jl:403-407
+  } else if (!tr_on) {  // solve.jl:436-445
+    B200_TRY(update_u(nw, 1.0, &objective, &du_norm));
+    nw->bytes += 5.0 * (8.0 * (double)nw->n);
+  } else {
+    B200_TRY(trust_region_step(nw, have_dJJd, dJJd, &accepted, &objective, &du_norm));
+  }
+  b200_trace_rec t = {};
+  t.accepted = accepted; t.lin_iters = gs.iters; t.lin_status = gs.status; t.lin_rnorm = gs.rnorm;
+  t.trust_radius = ls_on ? alpha : (o.descent == B200_DESCENT_PSEUDO_TRANSIENT) ? 1.0 / nw->alpha_inv : nw->trust_region;
+  return step_end(nw, objective, du_norm, t);
 }
 
 // CommonSolve.step! (NonlinearSolveBase/src/solve.jl:835-858): one step, the counters, and the wall-clock limit
