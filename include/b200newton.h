@@ -110,8 +110,10 @@ enum { B200_QN_UPDATE_GOOD_BROYDEN = 0, B200_QN_UPDATE_BAD_BROYDEN = 1, B200_QN_
    (an n-vector, any n): du = -f ./ J, J += ((df - J du) ./ (J^2 du^2)) .* du .* J^2, IllConditionedJacobianReset (any zero on the diagonal) */
 /* built-in preconditioners (LinearSolve `precs(A, p)`, large_systems.md:244-316): inverse of the 2x2 species blocks, or one
    geometric-multigrid V-cycle of the Brusselator Jacobian (the tutorial's AlgebraicMultigrid ruge_stuben / smoothed_aggregation) */
+/* ILU0: incomplete LU with zero fill of the assembled sparse Jacobian (b200_ilu0_*), refactorised with every fresh Jacobian;
+   needs linsolve = SPARSE_GMRES and works on any problem with a pattern (built-in or a callback's jac_prototype) */
 enum { B200_PRECOND_NONE = 0, B200_PRECOND_BLOCK_JACOBI_LEFT = 1, B200_PRECOND_BLOCK_JACOBI_RIGHT = 2,
-       B200_PRECOND_MULTIGRID_LEFT = 3, B200_PRECOND_MULTIGRID_RIGHT = 4 };
+       B200_PRECOND_MULTIGRID_LEFT = 3, B200_PRECOND_MULTIGRID_RIGHT = 4, B200_PRECOND_ILU0_LEFT = 5, B200_PRECOND_ILU0_RIGHT = 6 };
 enum { B200_FORCING_NONE = 0, B200_FORCING_EW2 = 1 };
 /* termination modes (public.jl:300-407, termination_conditions.jl:243-372); `du` = f(u).  The three AbsNorm modes keep
    their round-1 values; Norm / Rel / RelNorm / Abs / RelNormSafe / RelNormSafeBest follow */
@@ -360,6 +362,23 @@ int32_t b200_sparse_lu_destroy(b200_sparse_lu* lu);
 int32_t b200_sparse_lu_bandwidth(b200_sparse_lu* lu, int64_t* kl_host, int64_t* ku_host);
 int32_t b200_sparse_lu_factor(b200_sparse_lu* lu, const double* nzval_dev, int32_t* info_host);   /* info > 0: zero pivot at that column (1-based) */
 int32_t b200_sparse_lu_solve(b200_sparse_lu* lu, const double* b_dev, double* x_dev);            /* x = A^-1 b (x may alias b) */
+
+/* ---------------------------------------------------------------- ILU(0) preconditioner of an assembled sparse matrix
+ * Incomplete LU with the sparsity pattern of A (no fill, no pivoting): the first `precs` of large_systems.md:244-316.
+ * Symbolic phase on the host, once per pattern: CSR view with int32 indices (n, nnz < 2^31), diagonal positions, level sets
+ * of the strictly lower and strictly upper patterns.  Factorisation and solve run on the device, level by level in one
+ * cooperative launch each; results are bit-reproducible.  A row without a structural diagonal fails create with
+ * B200_ERR_INVALID (the message names the row). */
+typedef struct b200_ilu0 b200_ilu0;
+int32_t b200_ilu0_create(b200_ctx* ctx, int64_t n, const int64_t* colptr_host, const int64_t* rowval_host, int32_t index_base, b200_ilu0** ilu);
+int32_t b200_ilu0_destroy(b200_ilu0* ilu);
+int32_t b200_ilu0_levels(b200_ilu0* ilu, int32_t* lower_host, int32_t* upper_host);   /* level counts of the forward / backward sweep */
+int32_t b200_ilu0_factor(b200_ilu0* ilu, const double* nzval_dev, int32_t* info_host);  /* info > 0: zero or non-finite pivot u_ii at that row (1-based) */
+int32_t b200_ilu0_solve(b200_ilu0* ilu, const double* b_dev, double* x_dev);           /* x = U^-1 L^-1 b, L unit lower (x may alias b) */
+/* the packed factors in the caller's CSC order: L strictly below the diagonal (unit diagonal implied), U on and above it */
+int32_t b200_ilu0_export(b200_ilu0* ilu, double* nzval_out_dev);
+/* an operator applying U^-1 L^-1, for b200_gmres_set_precond; it borrows the handle (destroy the operator first) */
+int32_t b200_ilu0_linop(b200_ilu0* ilu, b200_linop** op);
 
 /* ---------------------------------------------------------------- Newton driver (a4, a7, a8, a9) */
 void b200_newton_opts_default(b200_newton_opts* opts);

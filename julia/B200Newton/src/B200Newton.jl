@@ -493,8 +493,13 @@ Brusselator Jacobian (large_systems.md:244-316 hands IncompleteLU.ilu / Algebrai
 abstract type B200Preconditioner end
 struct B200BlockJacobi <: B200Preconditioner end
 struct B200Multigrid <: B200Preconditioner end
+"""`B200ILU0()`: incomplete LU with zero fill of the assembled sparse Jacobian.  It factors the concrete matrix, so it is offered
+on the whole-solve path only: `B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :ilu0_left | :ilu0_right)`."""
+struct B200ILU0 <: B200Preconditioner end
 precond_kind(::B200BlockJacobi) = Int32(1)      # B200_PRECOND_BLOCK_JACOBI_LEFT (LEFT / RIGHT of a family name the same operator)
 precond_kind(::B200Multigrid) = Int32(3)        # B200_PRECOND_MULTIGRID_LEFT
+precond_op(::B200ILU0, ::Problem, ::B200Vector) = throw(ArgumentError(
+    "B200ILU0 needs the concrete sparse Jacobian: use B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :ilu0_left) (or :ilu0_right)"))
 function precond_op(P::B200Preconditioner, prob::Problem, u::B200Vector)
     op = Ref{Ptr{Cvoid}}(C_NULL)
     check(prob.ctx.handle, @ccall libb200.b200_linop_precond(prob.handle::Ptr{Cvoid}, u.ptr::Ptr{Float64}, precond_kind(P)::Int32, op::Ref{Ptr{Cvoid}})::Int32)
@@ -536,7 +541,7 @@ const _DESCENT = (newton = 0, pseudo_transient = 1, levenberg_marquardt = 2, bro
 const _QN_INIT = (identity = 0, true_jacobian = 1, low_rank = 2)
 const _QN_UPDATE = (good_broyden = 0, bad_broyden = 1, klement = 2)
 const _TR_SCHEMES = (simple = 0, nlsolve = 1, nocedal_wright = 2, hei = 3, yuan = 4, fan = 5, bastin = 6)
-const _PRECS = (none = 0, block_jacobi_left = 1, block_jacobi_right = 2, multigrid_left = 3, multigrid_right = 4)
+const _PRECS = (none = 0, block_jacobi_left = 1, block_jacobi_right = 2, multigrid_left = 3, multigrid_right = 4, ilu0_left = 5, ilu0_right = 6)
 const _TERMINATION = (abs_norm_safe_best = 0, abs_norm = 1, abs_norm_safe = 2, norm = 3, rel = 4, rel_norm = 5, abs = 6,
     rel_norm_safe = 7, rel_norm_safe_best = 8)
 
@@ -669,7 +674,7 @@ function SciMLBase.__solve(ens::SciMLBase.AbstractEnsembleProblem, alg::B200Newt
     return SciMLBase.EnsembleSolution(sols, time() - t0, converged)
 end
 
-export Context, B200Vector, brusselator, brusselator_function, initial_condition, B200GMRES, B200BlockJacobi, B200Multigrid,
+export Context, B200Vector, brusselator, brusselator_function, initial_condition, B200GMRES, B200BlockJacobi, B200Multigrid, B200ILU0,
     B200NewtonKrylov, EnsembleB200, nccl_unique_id, device_count
 
 end # module

@@ -26,6 +26,7 @@ LINSOLVE_GMRES, LINSOLVE_DENSE_LU, LINSOLVE_SPARSE_GMRES, LINSOLVE_SPARSE_LU = 0
 JVP_EXACT, JVP_FINITE_DIFF = 0, 1
 GLOB_NONE, GLOB_TRUST_REGION, GLOB_LINESEARCH = 0, 1, 2
 PRECOND_NONE, PRECOND_BLOCK_JACOBI_LEFT, PRECOND_BLOCK_JACOBI_RIGHT, PRECOND_MULTIGRID_LEFT, PRECOND_MULTIGRID_RIGHT = 0, 1, 2, 3, 4
+PRECOND_ILU0_LEFT, PRECOND_ILU0_RIGHT = 5, 6
 DESCENT_NEWTON, DESCENT_PSEUDO_TRANSIENT, DESCENT_LEVENBERG_MARQUARDT, DESCENT_BROYDEN = 0, 1, 2, 3
 QN_INIT_IDENTITY, QN_INIT_TRUE_JACOBIAN, QN_INIT_LOW_RANK = 0, 1, 2
 QN_UPDATE_GOOD_BROYDEN, QN_UPDATE_BAD_BROYDEN, QN_UPDATE_KLEMENT = 0, 1, 2
@@ -163,6 +164,13 @@ SIGNATURES = {
     "b200_sparse_lu_bandwidth": (I32, [P, PI64, PI64]),
     "b200_sparse_lu_factor": (I32, [P, P, PI32]),
     "b200_sparse_lu_solve": (I32, [P, P, P]),
+    "b200_ilu0_create": (I32, [P, I64, P, P, I32, PP]),
+    "b200_ilu0_destroy": (I32, [P]),
+    "b200_ilu0_levels": (I32, [P, PI32, PI32]),
+    "b200_ilu0_factor": (I32, [P, P, PI32]),
+    "b200_ilu0_solve": (I32, [P, P, P]),
+    "b200_ilu0_export": (I32, [P, P]),
+    "b200_ilu0_linop": (I32, [P, PP]),
     "b200_gmres_solve": (I32, [P, P, P, P, C.POINTER(GmresStats)]),
     "b200_dense_jac_fill": (I32, [P, P, P, I64]),
     "b200_getrf": (I32, [P, I64, P, I64, P, PI32]),

@@ -412,6 +412,21 @@ class Multigrid:
         return op
 
 
+class ILU0:
+    """Preconditioner for `KrylovJL_GMRES(precs = ...)` on the concrete sparse Jacobian: the incomplete LU with zero fill of
+    the assembled J, refactorised with every fresh Jacobian — the first `precs` of docs/src/tutorials/large_systems.md:244-316
+    (`IncompleteLU.ilu(W, τ = 50.0)` there; here no threshold, the pattern of J).  Needs `concrete_jac = True` or a sparse
+    prototype, and serves any problem with a pattern, including a user residual with `jac_prototype`."""
+
+    def __init__(self, side="left"):
+        assert side in ("left", "right")
+        self.side = side
+
+    @property
+    def code(self):
+        return abi.PRECOND_ILU0_LEFT if self.side == "left" else abi.PRECOND_ILU0_RIGHT
+
+
 class LUFactorization:
     needs_concrete_A = True
 
@@ -450,6 +465,47 @@ class SparseBandLU:
         x = x or self.ctx.zeros(self.n)
         check(self.ctx.handle, lib().b200_sparse_lu_solve(self._h, b.ptr, x.ptr))
         return x
+
+
+class SparseILU0:
+    """Direct handle on the device ILU(0) of a CSC pattern (colptr, rowval host arrays, 1-based by default): `factor(nzval)`
+    returns 0 or the 1-based row of a zero / non-finite pivot, `solve(b)` applies U^-1 L^-1, `factors()` returns the packed
+    factors in the pattern's CSC order (L strictly below the diagonal, unit diagonal implied; U on and above it)."""
+
+    def __init__(self, ctx, n, colptr, rowval, index_base=1):
+        self.ctx, self.n = ctx, n
+        colptr = np.ascontiguousarray(colptr, dtype=np.int64)
+        rowval = np.ascontiguousarray(rowval, dtype=np.int64)
+        self.nnz = int(colptr[n] - colptr[0])
+        self._h = C.c_void_p()
+        check(ctx.handle, lib().b200_ilu0_create(ctx.handle, n, colptr.ctypes.data_as(C.c_void_p), rowval.ctypes.data_as(C.c_void_p), index_base, C.byref(self._h)))
+        self._fin = ctx._adopt(weakref.finalize(self, lib().b200_ilu0_destroy, self._h))
+
+    def levels(self):
+        lo, up = C.c_int32(0), C.c_int32(0)
+        check(self.ctx.handle, lib().b200_ilu0_levels(self._h, C.byref(lo), C.byref(up)))
+        return lo.value, up.value
+
+    def factor(self, nzval):
+        info = C.c_int32(0)
+        check(self.ctx.handle, lib().b200_ilu0_factor(self._h, nzval.ptr, C.byref(info)))
+        return info.value
+
+    def solve(self, b, x=None):
+        x = x or self.ctx.zeros(self.n)
+        check(self.ctx.handle, lib().b200_ilu0_solve(self._h, b.ptr, x.ptr))
+        return x
+
+    def factors(self, out=None):
+        out = out or self.ctx.zeros(self.nnz)
+        check(self.ctx.handle, lib().b200_ilu0_export(self._h, out.ptr))
+        return out
+
+    def linop(self):
+        """A borrowed-by-GMRES operator handle applying U^-1 L^-1 (destroy it with b200_linop_destroy before this handle)."""
+        op = C.c_void_p()
+        check(self.ctx.handle, lib().b200_ilu0_linop(self._h, C.byref(op)))
+        return op
 
 
 class AutoForwardDiff:

@@ -216,7 +216,7 @@ constexpr int32_t B200I_ENS_RC_DEFERRED = -7;  // batched ensemble kernel -> hos
 
 struct b200_linop {
   b200_ctx* ctx;
-  int32_t kind;  // 0 problem-jvp, 1 csc, 2 dense, 3 callback, 4 sparse_jac
+  int32_t kind;  // LINOP_*
   int64_t n;
   b200_problem* prob;
   const double* u;
@@ -233,8 +233,10 @@ struct b200_linop {
   b200_mg* mg;   // LINOP_MULTIGRID: the hierarchy (owned when owns_mg)
   int32_t owns_mg;
   int64_t *csr_rowptr, *csr_col, *csr_map;  // LINOP_CSC: row view of the pattern (owned), built once so that y = A x is a deterministic gather
+  b200_ilu0* ilu;  // LINOP_ILU0: the factors (borrowed)
 };
-enum { LINOP_PROBLEM = 0, LINOP_CSC = 1, LINOP_DENSE = 2, LINOP_CALLBACK = 3, LINOP_SPARSE_JAC = 4, LINOP_BLOCK_JACOBI = 5, LINOP_MULTIGRID = 6 };
+enum { LINOP_PROBLEM = 0, LINOP_CSC = 1, LINOP_DENSE = 2, LINOP_CALLBACK = 3, LINOP_SPARSE_JAC = 4, LINOP_BLOCK_JACOBI = 5, LINOP_MULTIGRID = 6,
+       LINOP_ILU0 = 7 };
 
 // internal (non-ABI) helpers implemented across the .cu files
 // Host callbacks run user device code on streams the library knows nothing about (its own stream is non-blocking): drain

@@ -62,6 +62,8 @@ struct b200_newton {
   b200_sparse_jac* sj;
   double* nzval;
   b200_sparse_lu* slu;  // LINSOLVE_SPARSE_LU: band factorisation of the assembled Jacobian
+  b200_ilu0* ilu;       // PRECOND_ILU0_*: incomplete LU of the assembled Jacobian, refactorised with every fresh J
+  int32_t ilu_info;     // its last factorisation: 0, or the 1-based row of a zero / non-finite pivot
   // LevenbergMarquardt: J'J + lambda D'D (factored in place), the running diagonal D'D, velocity / acceleration, previous velocity, J' f
   double *lmA, *lm_dtd, *lm_v, *lm_a, *lm_vold, *lm_rhs;
   double lm_lambda, lm_lambda_factor, lm_norm_v_old, lm_loss_old;
@@ -226,9 +228,12 @@ int32_t b200_newton_destroy(b200_newton* nw) {
   if (nw->mg) b200i_mg_destroy(nw->mg);
   if (nw->sj) b200_sparse_jac_destroy(nw->sj);
   if (nw->slu) b200_sparse_lu_destroy(nw->slu);
+  if (nw->ilu) b200_ilu0_destroy(nw->ilu);
   delete nw;
   return B200_OK;
 }
+
+static bool ilu0_precond(const b200_newton_opts& o) { return o.precond == B200_PRECOND_ILU0_LEFT || o.precond == B200_PRECOND_ILU0_RIGHT; }
 
 // the buffers and sub-solvers b200_newton_create builds for the options; on failure the caller destroys the partial driver
 static int32_t newton_setup(b200_newton* nw) {
@@ -288,6 +293,7 @@ static int32_t newton_setup(b200_newton* nw) {
     B200_TRY(dev_alloc(nw, &nw->nzval, (size_t)nnz, "sparse Jacobian: the nonzero values do not fit in device memory"));
     // sparse direct route (linsolve = nothing on a sparse prototype): symbolic phase once, like LinearSolve's cache
     if (o.linsolve == B200_LINSOLVE_SPARSE_LU) B200_TRY(b200_sparse_lu_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->slu));
+    if (ilu0_precond(o)) B200_TRY(b200_ilu0_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->ilu));
     nw->op.kind = LINOP_SPARSE_JAC; nw->op.sj = nw->sj; nw->op.nzval = nw->nzval;
   } else {
     return ctx->fail(B200_ERR_INVALID, "unknown linsolve kind", __FILE__, __LINE__);
@@ -313,11 +319,20 @@ int32_t b200_newton_create(b200_problem* prob, const b200_newton_opts* opts, b20
                           (opts->qn_update_rule == B200_QN_UPDATE_KLEMENT && opts->qn_init_jacobian == B200_QN_INIT_IDENTITY))),
                "newton_create: descent must be Newton, PseudoTransient (without a trust region), LevenbergMarquardt (dense concrete Jacobian, its own trust region) or "
                "Broyden (no globalisation, n <= 65535, init_jacobian = true_jacobian needs the dense LU)");
-  B200_REQUIRE(ctx, opts->precond == B200_PRECOND_NONE ||
-                        ((opts->linsolve == B200_LINSOLVE_GMRES || opts->linsolve == B200_LINSOLVE_SPARSE_GMRES) &&
-                         (prob->kind == B200_PROB_BRUSS2D || prob->kind == B200_PROB_BRUSS3D)),
-               "newton_create: the built-in preconditioners need a Krylov linsolve and a built-in Brusselator problem");
-  B200_REQUIRE(ctx, opts->precond >= B200_PRECOND_NONE && opts->precond <= B200_PRECOND_MULTIGRID_RIGHT, "newton_create: unknown preconditioner");
+  B200_REQUIRE(ctx, opts->precond >= B200_PRECOND_NONE && opts->precond <= B200_PRECOND_ILU0_RIGHT, "newton_create: unknown preconditioner");
+  if (ilu0_precond(*opts)) {
+    // ILU(0) factors the assembled sparse Jacobian, so any problem with a pattern qualifies; the SER shift of PseudoTransient
+    // changes every step and would need a refactorisation every step, as on the sparse direct route
+    B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_SPARSE_GMRES,
+                 "newton_create: the ILU0 preconditioner factors the assembled sparse Jacobian: use concrete_jac = true (linsolve B200_LINSOLVE_SPARSE_GMRES)");
+    if (opts->descent == B200_DESCENT_PSEUDO_TRANSIENT)
+      return ctx->fail(B200_ERR_UNSUPPORTED, "newton_create: PseudoTransient with the ILU0 preconditioner is not offered (use block-Jacobi, multigrid or no preconditioner)", __FILE__, __LINE__);
+  } else {
+    B200_REQUIRE(ctx, opts->precond == B200_PRECOND_NONE ||
+                          ((opts->linsolve == B200_LINSOLVE_GMRES || opts->linsolve == B200_LINSOLVE_SPARSE_GMRES) &&
+                           (prob->kind == B200_PROB_BRUSS2D || prob->kind == B200_PROB_BRUSS3D)),
+                 "newton_create: the built-in preconditioners need a Krylov linsolve and a built-in Brusselator problem");
+  }
   b200_newton* nw = new b200_newton();
   nw->ctx = ctx; nw->prob = prob; nw->o = *opts; nw->n = prob->n;
   nw->abstol = opts->abstol > 0 ? opts->abstol : 3.0e-13;  // common_defaults.jl:44-48
@@ -742,7 +757,10 @@ static int32_t refresh_jacobian(b200_newton* nw, bool* fresh) {
   nw->res.njacs += 1;
   nw->have_factor = 0;
   if (nw->o.linsolve == B200_LINSOLVE_DENSE_LU) return b200_dense_jac_fill(nw->prob, nw->u, nw->Jdense, nw->n);  // written straight into the LU workspace (K10: no copyto!)
-  return b200_sparse_jac_fill(nw->sj, nw->u, nw->nzval);
+  B200_TRY(b200_sparse_jac_fill(nw->sj, nw->u, nw->nzval));
+  // precs(A, p) on the new A; not an NLStats factorisation (LinearSolve's Krylov route counts none)
+  if (nw->ilu) B200_TRY(b200_ilu0_factor(nw->ilu, nw->nzval, &nw->ilu_info));
+  return B200_OK;
 }
 
 // What precedes each linear solve: the PseudoTransient shift (its SER update once per step, on the first attempt) and the
@@ -825,16 +843,19 @@ static int32_t linear_solve(b200_newton* nw, bool fresh, bool* ok, b200_gmres_st
   } else {
     // `linu` aliases the du buffer: it is the initial guess only when warm_start is requested
     if (o.gmres.warm_start) CUDA_TRY(ctx, cudaMemcpyAsync(nw->xlin, nw->du, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (nw->ilu && nw->ilu_info != 0) { *ok = false; return B200_OK; }  // zero pivot: a failed solve, retried with a fresh Jacobian
     if (o.precond != B200_PRECOND_NONE) {  // precs(A, p): rebuilt from the current iterate, like update_A! does for Pl / Pr
       memset(&nw->prec, 0, sizeof(nw->prec));
       nw->prec.ctx = ctx; nw->prec.n = n; nw->prec.prob = nw->prob; nw->prec.u = nw->u;
       if (nw->mg) {
         nw->prec.kind = LINOP_MULTIGRID; nw->prec.mg = nw->mg;
         if (fresh) B200_TRY(b200i_mg_setup(nw->mg, nw->u));  // coarse operators follow the linearisation point
+      } else if (nw->ilu) {
+        nw->prec.kind = LINOP_ILU0; nw->prec.ilu = nw->ilu;  // factorised by refresh_jacobian
       } else {
         nw->prec.kind = LINOP_BLOCK_JACOBI;
       }
-      const bool left = o.precond == B200_PRECOND_BLOCK_JACOBI_LEFT || o.precond == B200_PRECOND_MULTIGRID_LEFT;
+      const bool left = o.precond == B200_PRECOND_BLOCK_JACOBI_LEFT || o.precond == B200_PRECOND_MULTIGRID_LEFT || o.precond == B200_PRECOND_ILU0_LEFT;
       B200_TRY(b200_gmres_set_precond(nw->gm, left ? &nw->prec : nullptr, left ? nullptr : &nw->prec));
     }
     B200_TRY(b200_gmres_solve(nw->gm, &nw->op, nw->fu, nw->xlin, gs));
