@@ -169,12 +169,16 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, unsigned bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity) {
+// gives up after 2^26 polls; sets *err (when given) so that the caller reports the timeout instead of using stale data
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity, int* err = nullptr) {
   const unsigned a = (unsigned)__cvta_generic_to_shared(bar);
   unsigned done = 0, spins = 0;
   while (!done) {
     asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(a), "r"(parity) : "memory");
-    if (++spins > (1u << 26)) break;
+    if (++spins > (1u << 26)) {
+      if (err) *err = 1;
+      break;
+    }
   }
 }
 __device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, unsigned bytes, uint64_t* bar) {
@@ -186,6 +190,13 @@ __device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, 
 __device__ __forceinline__ void l2_bulk_prefetch(const void* gsrc, unsigned bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
 }
+// 16-byte global -> shared copy (non-bulk cp.async, L2 only); completes into the thread's current cp.async group
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
+}
+// orders this thread's generic-proxy accesses to shared memory (loads, stores, completed non-bulk cp.async) before later
+// async-proxy (TMA) accesses; place it before the barrier after which one thread issues the bulk copy
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- flag-in-word cross-CTA exchange (the idea of NCCL's LL protocol): a 64-bit value travels as two 64-bit words of
 //      {32 data bits | 32-bit epoch << 32}, written by ONE 16-byte store, so a reader that sees the expected epoch in both words

@@ -535,8 +535,25 @@ __device__ __forceinline__ void resident_givens_tail(const ResidentParams& P, do
 // in every 64-bit word), one entry per polling thread; four table buffers rotate.
 // Capacity: at N = 100 on the 132 SMs of an H100 a CTA owns 15 152 rows, and w plus three whole vectors (485 KB) exceed what
 // one SM holds (64K registers + 227 KB of shared memory).  The shared-memory stages therefore keep the first `qs` row pairs of
-// every thread (the prefix of the CTA's rows that fits beside the annex); the pairs q >= qs of those two stages are read from
-// global memory at each of their two uses — one step apart, so the second read mostly hits the 50 MB L2.
+// every thread (the prefix of the CTA's rows that fits beside the annex); the pairs q >= qs of those two stages (the global
+// tail, 9 per thread at N = 100) are needed at each of their two uses, the dot sweep of step t-1 and the update sweep of step t.
+// With the register file full, a tail pair read straight from global memory is one dependent L2 round trip; instead the tail
+// is copied by 16-byte cp.async, all pairs in flight together, into stage slots the thread has released (R3_SLOTGET):
+//   update sweep of v_t (shared-memory role): once pairs 0 .. R3_TAIL_AT-1 are applied, their slots of v_t's own stage are
+//     free; the tail lands there while pairs R3_TAIL_AT .. qs-1 are applied, and is applied last (the pair order is unchanged);
+//   dot sweep of v_{t+1} when it is stage 0's (t = 2 mod 3): the tail lands in stage 1, released by v_{t-1} one step before,
+//     whose refill with v_{t+2} waits until every thread has passed the barrier after that dot sweep (an L2 prefetch of the
+//     whole of v_{t+2} keeps the old place).  The dot sweep of stage 1's vectors has no released slots (stage 0 holds v_t,
+//     the annex v_{t+2}) and reads its tail from global memory.
+// Which tail pairs have a slot: r3_update_slot / r3_dot_slot below; the others are read directly.
+// cp.async groups of a thread, in commit order over one rotation (steps t = 0, 1, 2 mod 3):
+//   end of a role-2 step:  R, the register stage's annex of v_{t+3};
+//   role-0 step:           U0, the update-sweep tail of v_t; its wait (inside the sweep) also completes R, issued half a
+//                          step earlier;
+//   role-1 step:           the wait at its start (register stage of v_{t+1}) finds R complete; U1 is committed and waited
+//                          inside the update sweep; D, the dot-sweep tail of v_{t+2}, is committed at its end;
+//   role-2 step:           D alone is pending at the wait inside the dot sweep.
+// At most two groups are ever pending; the only wait that completes a group other than its sweep's own is U0's (R).
 constexpr int R3_RP = 30;            // row pairs per thread
 constexpr int R3_ROWS = 2 * R3_RP;   // 60 rows per thread -> at most 15360 rows (7680 cells) per CTA
 constexpr int R3_RPR = 16;           // pairs of the third stage held in registers; the last R3_RP - R3_RPR pairs of each thread
@@ -589,9 +606,8 @@ struct R3Ctx {
 };
 
 // The shared-memory stages hold the CTA's rows [0, 2 * R3_THREADS * qs): a prefix of the first species' segment, or all of it
-// and a prefix of the second species' segment.  The rows past the stage are read from global memory, one dependent round trip
-// per row pair (the register file is full, nothing is hoisted); they are prefetched into L2 here, two steps before the dot
-// sweep that first reads them, so that round trip ends in L2 instead of HBM.
+// and a prefix of the second species' segment.  The rows past the stage (the global tail) are prefetched into L2 here, so that
+// their copies into stage slots and the direct reads of the stage-1 dot sweep end in L2 instead of HBM.
 __device__ __forceinline__ void r3_issue_smem(const ResidentParams& P, const R3Ctx& cx, uint64_t* mbar, int t, int stage) {
   if (threadIdx.x == 0 && cx.nrow > 0) {
     const double* src = P.V[t % cx.k];
@@ -620,6 +636,48 @@ __device__ __forceinline__ void r3_issue_smem(const ResidentParams& P, const R3C
     else z_ = __ldg(reinterpret_cast<const double2*>((gp) + (lr) + (((lr) >= lims) ? hop : (int64_t)0)));                        \
     o0 = z_.x; o1 = z_.y;                                                                                                         \
   } while (0)
+// the same when tail pair q, if `slot`, was copied by r3_tail_copy into slot q - qs of stage `tp` (this thread's first
+// element); the thread's cp.async groups are waited for at the first of them, q = qs
+#define R3_SLOTGET(q, lr, sp, tp, slot, gp, o0, o1)                                                                             \
+  do {                                                                                                                            \
+    double2 z_;                                                                                                                   \
+    if ((q) < cx.qs) z_ = *reinterpret_cast<const double2*>((sp) + (lr));                                                         \
+    else if (slot) {                                                                                                              \
+      if ((q) == cx.qs) asm volatile("cp.async.wait_group 0;" ::: "memory");                                                     \
+      z_ = *reinterpret_cast<const double2*>((tp) + (lr) - 2 * R3_THREADS * cx.qs);                                               \
+    } else z_ = __ldg(reinterpret_cast<const double2*>((gp) + (lr) + (((lr) >= lims) ? hop : (int64_t)0)));                     \
+    o0 = z_.x; o1 = z_.y;                                                                                                         \
+  } while (0)
+// L2 prefetch of all of this CTA's rows of vector t (both species' segments)
+__device__ __forceinline__ void r3_prefetch_l2(const ResidentParams& P, const R3Ctx& cx, int t) {
+  if (threadIdx.x == 0 && cx.nrow > 0) {
+    const double* src = P.V[t % cx.k] + (int64_t)cx.b * P.cpc;
+    l2_bulk_prefetch(src, (unsigned)cx.ncell * 8u);
+    l2_bulk_prefetch(src + P.NC, (unsigned)cx.ncell * 8u);
+  }
+}
+// Slots of the global tail (pairs q >= qs at slot q - qs, nslot <= qs of them): every released slot in the dot sweep of a
+// stage-0 vector; in an update sweep, the slots of pairs 0 .. R3_TAIL_AT-1, and only when the copy is issued before the first
+// tail pair is needed (qs >= R3_TAIL_AT).  The update sweep issues its copy at one compile-time place, after pair R3_TAIL_AT-1:
+// a place that depends on qs at run time costs registers the kernel does not have (it spills).  R3_TAIL_AT = 9 covers the
+// whole tail of the stock split at N = 100 (qs = 21 of 30 pairs) and of every split from qs = 21 on.
+constexpr int R3_TAIL_AT = 9;
+// whether tail pair q (>= qs, compile-time after unrolling) sits in a slot, written as comparisons of qs with constants
+// (a slot bound held in a register costs one the kernel does not have)
+__device__ __forceinline__ bool r3_dot_slot(const R3Ctx& cx, int q) { return cx.qs > q / 2; }  // q < 2 qs
+__device__ __forceinline__ bool r3_update_slot(const R3Ctx& cx, int q) { return cx.qs >= R3_TAIL_AT && cx.qs > q - R3_TAIL_AT; }
+// this thread's global-tail pairs q = qs .. qs + nslot - 1 of a vector (`gp` = its first element of this thread, lim / lims /
+// hop as in r3_issue_regs) -> slots 0 .. nslot-1 of a stage (`ts` = the stage + 2 * tid), one cp.async group.  Every source
+// lies in this CTA's rows of one species' segment; sources and slots are 16-byte aligned (even offsets of aligned bases).
+// Call only when the thread has a tail pair (lim > 2 * R3_THREADS * qs): the group it commits is waited on in R3_SLOTGET.
+__device__ __forceinline__ void r3_tail_copy(const R3Ctx& cx, const double* gp, double* ts, int nslot, int lim, int lims, int64_t hop) {
+  for (int j = 0; j < nslot; ++j) {
+    const int lr = 2 * R3_THREADS * (cx.qs + j);
+    if (lr >= lim) break;  // also ends the copy at pair R3_RP - 1
+    cp_async16(ts + 2 * R3_THREADS * j, gp + lr + ((lr >= lims) ? hop : (int64_t)0));
+  }
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
 __device__ __forceinline__ void r3_issue_regs(const ResidentParams& P, const R3Ctx& cx, int t, double (&vr)[R3_VR]) {
   // thread-relative form (constant offsets, two per-thread limits) so that nothing per-q stays live across the step
   const double* src = P.V[t % cx.k] + (int64_t)cx.b * P.cpc + 2 * (int)threadIdx.x;
@@ -770,14 +828,17 @@ static_assert(R3_THREADS == 8 * 32 && R3_POLLERS == 5 * 32, "sum8 / sum5 add the
 __device__ __forceinline__ double sum8(const double* r) { return ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7])); }
 __device__ __forceinline__ double sum5(const double* g) { return ((g[0] + g[1]) + (g[2] + g[3])) + g[4]; }
 
-template <int ROLE>
+// TAIL: this CTA has a global tail (rows past its stages).  Without one (N <= 88 on an H100) the step compiles to the plain
+// three-stage rotation, with none of the tail's branches in its sweeps.
+template <int ROLE, bool TAIL>
 __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3GShared& sh, int t, double (&w)[R3_ROWS], double (&vr)[R3_VR]) {
   constexpr int NEXT = (ROLE + 1) % 3;
   const int tid = threadIdx.x;
   const int par = t & 1;
   const int lim = cx.nrow - 2 * tid;                       // row pair q of this thread exists iff 2 * R3_THREADS * q < lim
-  const double* sc = (ROLE == 0 ? cx.stage0 : cx.stage1) + 2 * tid;   // current vector if it lives in shared memory
+  double* const sc = (ROLE == 0 ? cx.stage0 : cx.stage1) + 2 * tid;   // current vector if it lives in shared memory
   const double* sn = (NEXT == 0 ? cx.stage0 : cx.stage1) + 2 * tid;   // next vector if it lives in shared memory
+  const bool tail = TAIL && lim > 2 * R3_THREADS * cx.qs;  // this thread has a global tail
   const bool more = t + 1 < cx.total;
   const int i = t % cx.k;
   const int lims = cx.ncell - 2 * tid;
@@ -788,7 +849,7 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
   unsigned long long ea0, ea1;
   r3g_poll_issue(pollbuf, cx.b, cx.G, ea0, ea1);
   if (more) {
-    if (NEXT != 2 && cx.nrow > 0) mbar_wait(&sh.mbar[NEXT], (unsigned)(((t + 1) / 3) & 1));
+    if (NEXT != 2 && cx.nrow > 0) mbar_wait(&sh.mbar[NEXT], (unsigned)(((t + 1) / 3) & 1), P.err);
     if (NEXT == 2) asm volatile("cp.async.wait_group 0;" ::: "memory");
     double da = 0.0, dc = 0.0;
     if (i + 1 == cx.k) {  // wrap-around into the next Gram-Schmidt pass: <v_0, v_{k-1}> is not stored, take it in the sweep
@@ -798,6 +859,7 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
         if (lr < lim) {
           double x0, x1, y0, y1;
           if (NEXT == 2) { R3_VRGET(q, x0, x1); }
+          else if (NEXT == 0) { R3_SLOTGET(q, lr, sn, cx.stage1 + 2 * tid, TAIL && r3_dot_slot(cx, q), vnext, x0, x1); }
           else { R3_SMGET(q, lr, sn, vnext, x0, x1); }
           if (ROLE == 2) { R3_VRGET(q, y0, y1); }
           else { R3_SMGET(q, lr, sc, vcur, y0, y1); }
@@ -814,6 +876,7 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
         if (lr < lim) {
           double x0, x1;
           if (NEXT == 2) { R3_VRGET(q, x0, x1); }
+          else if (NEXT == 0) { R3_SLOTGET(q, lr, sn, cx.stage1 + 2 * tid, TAIL && r3_dot_slot(cx, q), vnext, x0, x1); }
           else { R3_SMGET(q, lr, sn, vnext, x0, x1); }
           da = fma(x0, w[2 * q], da); db = fma(x1, w[2 * q + 1], db);
         }
@@ -826,7 +889,14 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
   // Gram sub-diagonal entry <v_i, v_{i-1}>, stored when v_i was created: fetched by the spare polling thread
   if (tid == R3_SPARE_POLLER) sh.gC[par][R3_POLLERS / 32] = (i > 0) ? __ldg(P.gsub + i) : 0.0;
   r3g_poll_finish(pollbuf, cx.b, cx.G, P.epoch_base + (unsigned)t + 1u, P.err, i == 0 && t > 0, ea0, ea1, sh.gA[par], sh.gC[par]);
+  // a deferred refill of stage 1 follows: its slots took the cp.async tail of v_{t+1} (completed in the sweep above); the
+  // async-proxy copy into them is ordered after those writes by this fence in every writing thread and the barrier (PTX ISA,
+  // memory consistency model, "Proxies": a non-bulk cp.async is a generic-proxy write, cp.async.bulk is performed in the async
+  // proxy, and accesses to one location through both need a fence.proxy.async between them).  A thread that only loaded from
+  // the stage needs the barrier alone, as every refill always has.
+  if (ROLE == 2 && tail) fence_proxy_async_smem();
   __syncthreads();  // the only barrier of a register-role step
+  if (ROLE == 2 && TAIL && t + 2 < cx.total) r3_issue_smem(P, cx, sh.mbar, t + 2, 1);
   if (more && tid < 32) {  // warp 0: total of the eight warp partials in a fixed order, then publish for step t+1
     r3_post(P.slots + (size_t)((t + 1) & 3) * R3_BUF_WORDS, cx.b, sum8(sh.redA[par]), sum8(sh.redC[par]), P.epoch_base + (unsigned)(t + 1) + 1u);
   }
@@ -842,10 +912,11 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
       if (lr < lim) {
         double y0, y1;
         if (ROLE == 2) { R3_VRGET(q, y0, y1); }
-        else { R3_SMGET(q, lr, sc, vcur, y0, y1); }
+        else { R3_SLOTGET(q, lr, sc, sc, TAIL && r3_update_slot(cx, q), vcur, y0, y1); }
         w[2 * q] = fma(-h, y0, w[2 * q]);
         w[2 * q + 1] = fma(-h, y1, w[2 * q + 1]);
       }
+      if (ROLE != 2 && q + 1 == R3_TAIL_AT && cx.qs >= R3_TAIL_AT && tail) r3_tail_copy(cx, vcur, sc, R3_TAIL_AT, lim, lims, hop);
     }
   } else {  // last update of the Arnoldi step: ||w||^2 and <w, v_{k-1}> (next step's Gram sub-diagonal entry) ride along
     double nacc = 0.0, xacc = 0.0;
@@ -855,23 +926,28 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
       if (lr < lim) {
         double y0, y1;
         if (ROLE == 2) { R3_VRGET(q, y0, y1); }
-        else { R3_SMGET(q, lr, sc, vcur, y0, y1); }
+        else { R3_SLOTGET(q, lr, sc, sc, TAIL && r3_update_slot(cx, q), vcur, y0, y1); }
         const double w0 = fma(-h, y0, w[2 * q]), w1 = fma(-h, y1, w[2 * q + 1]);
         w[2 * q] = w0; w[2 * q + 1] = w1;
         nacc = fma(w0, w0, nacc); nacc = fma(w1, w1, nacc);
         xacc = fma(w0, y0, xacc); xacc = fma(w1, y1, xacc);
       }
+      if (ROLE != 2 && q + 1 == R3_TAIL_AT && cx.qs >= R3_TAIL_AT && tail) r3_tail_copy(cx, vcur, sc, R3_TAIL_AT, lim, lims, hop);
     }
     nacc = warp_sum(nacc);
     xacc = warp_sum(xacc);
     if ((tid & 31) == 0) { sh.redA[par ^ 1][tid >> 5] = nacc; sh.redC[par ^ 1][tid >> 5] = xacc; }  // parity of "step total"
   }
   if (cx.b == 0 && tid == 0) P.h[i] = (t < cx.k) ? h : P.h[i] + h;
-  if (ROLE != 2) {
+  if (ROLE == 0 || (ROLE == 1 && !TAIL)) {
     if (t + 3 < cx.total) {
-      __syncthreads();  // every thread is done with this shared-memory stage
+      if (tail) fence_proxy_async_smem();  // this step's cp.async tail of the stage before the bulk copy into it (see above)
+      __syncthreads();                     // every thread is done with this shared-memory stage
       r3_issue_smem(P, cx, sh.mbar, t + 3, ROLE);
     }
+  } else if (ROLE == 1) {  // stage 1 is refilled after the next dot sweep; until then its slots take the tail of v_{t+2}
+    if (t + 3 < cx.total) r3_prefetch_l2(P, cx, t + 3);
+    if (t + 2 < cx.total && tail) r3_tail_copy(cx, P.V[(t + 2) % cx.k] + (int64_t)cx.b * P.cpc + 2 * tid, sc, cx.qs, lim, lims, hop);
   } else if (t + 3 < cx.total) {
     r3_issue_regs(P, cx, t + 3, vr);
   }
@@ -910,7 +986,7 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
   const int lim = nrow - 2 * tid;
   if (total > 2) r3_issue_regs(P, cx, 2, vr);
   {
-    if (nrow > 0) mbar_wait(&sh.mbar[0], 0u);
+    if (nrow > 0) mbar_wait(&sh.mbar[0], 0u, P.err);
     const int lims = cx.ncell - 2 * tid;
     const int64_t hop = P.NC - cx.ncell;
     const double* g0 = P.V[0] + (int64_t)b * cpc + 2 * tid;
@@ -930,10 +1006,17 @@ __global__ void __launch_bounds__(R3_THREADS, 1) resident3g_arnoldi_kernel(Resid
     __syncthreads();
     if (tid < 32) r3_post(P.slots, b, sum8(sh.redA[1]), 0.0, P.epoch_base + 1u);
   }
+  const bool tailed = nrow > 2 * R3_THREADS * cx.qs;
   for (int t = 0; t < total; t += 3) {
-    r3g_step<0>(P, cx, sh, t, w, vr);
-    if (t + 1 < total) r3g_step<1>(P, cx, sh, t + 1, w, vr);
-    if (t + 2 < total) r3g_step<2>(P, cx, sh, t + 2, w, vr);
+    if (tailed) {
+      r3g_step<0, true>(P, cx, sh, t, w, vr);
+      if (t + 1 < total) r3g_step<1, true>(P, cx, sh, t + 1, w, vr);
+      if (t + 2 < total) r3g_step<2, true>(P, cx, sh, t + 2, w, vr);
+    } else {
+      r3g_step<0, false>(P, cx, sh, t, w, vr);
+      if (t + 1 < total) r3g_step<1, false>(P, cx, sh, t + 1, w, vr);
+      if (t + 2 < total) r3g_step<2, false>(P, cx, sh, t + 2, w, vr);
+    }
   }
   // ---- 3. ||w|| and <w, v_{k-1}> in one exchange (the last step left the warp partials in the scratch of parity
   //         `total`), Givens (CTA 0), normalise, store v_{k+1}
