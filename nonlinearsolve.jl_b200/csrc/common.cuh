@@ -91,6 +91,20 @@ enum { RED_DOT = 0, RED_SUMSQ = 1, RED_MAXABS = 2, RED_DIFFSQ = 3, RED_MIN = 4, 
 
 #define CHECK_LAUNCH(ctx) CUDA_TRY(ctx, cudaPeekAtLastError())
 
+// cooperative launch (every CTA co-resident, the guarantee of cudaLaunchCooperativeKernel), counted and timed like PLAUNCH
+template <typename... Params, typename... Args>
+int32_t coop_launch(b200_ctx* ctx, int kid, double bytes, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, Args... args) {
+  cudaLaunchAttribute coop;
+  coop.id = cudaLaunchAttributeCooperative;
+  coop.val.cooperative = 1;
+  const cudaLaunchConfig_t cfg = {grid, block, smem, ctx->stream, &coop, 1};
+  if (ctx->prof_on) ctx->prof_begin(kid, bytes);
+  CUDA_TRY(ctx, cudaLaunchKernelEx(&cfg, kernel, args...));
+  ctx->launches++;
+  if (ctx->prof_on) ctx->prof_end();
+  return B200_OK;
+}
+
 // ---------------------------------------------------------------- device helpers
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll

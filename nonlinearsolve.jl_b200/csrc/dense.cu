@@ -8,9 +8,9 @@
 // getrf structure (outer block NBO = 256 / 512, inner block NBI = 32):
 //   inner panel (32 columns): ONE cooperative kernel (`panel_coop_kernel`): every CTA keeps its rows of the panel in shared
 //       memory for all 32 columns; per column only the arg-max partials and two 32-double rows cross CTAs
-//   after an inner panel: TRSM + GEMM (K = 32) on the remaining columns of the outer panel
-//   after the outer panel: row interchanges applied to the columns left/right of it, block TRSM for U12, and the
-//       trailing update  A22 -= L21 U12  with K = NBO — the GEMM-shaped 2/3 n^3 flops — on the FP64 tensor cores
+//   after an inner panel: TRSM (`u12_fused_kernel`) + GEMM (K = 32) on the remaining columns of the outer panel
+//   after the outer panel: row interchanges applied to the columns left/right of it, TRSM for U12 (`u12_fused_kernel`), and
+//       the trailing update  A22 -= L21 U12  with K = NBO — the GEMM-shaped 2/3 n^3 flops — on the FP64 tensor cores
 //       (`gemm_sub_w8_kernel`: mma.sync.m8n8k4.f64 = DMMA.8x8x4 in SASS, the native FP64 MMA shape of sm_90a — m16n8k16
 //       compiles to eight of them; wgmma has no FP64 kind).  Look-ahead: the next panel's columns are updated first and
 //       the panel is factored on a second, HIGHEST-PRIORITY stream underneath the rest of the update.
@@ -20,11 +20,6 @@
 #include "common.cuh"
 #include <math.h>
 #include <algorithm>
-#include <vector>
-#include <cstdio>
-#include <cstdlib>
-#include <cooperative_groups.h>
-namespace cg = cooperative_groups;
 
 namespace {
 constexpr int NBO_DEFAULT = 256;  // outer block (GEMM K)
@@ -84,16 +79,6 @@ __global__ void __launch_bounds__(DT) unit_vector_kernel(int64_t n, int64_t j, d
 }
 
 // ------------------------------------------------------------------ panel factorisation (multi-CTA, column by column)
-struct PanelScratch {      // device scratch shared by the three panel kernels
-  double pmax[PS_MAX];     // per-CTA arg-max partials of the current column
-  int64_t pidx[PS_MAX];
-  double rowbuf[2][NBI];   // cooperative panel: pivot row / displaced row exchanged between CTAs
-  double inv_pivot;        // 1 / pivot of the current column (0 if the pivot is exactly zero)
-  int64_t piv;
-  int info;
-  int nparts;
-};
-
 __device__ __forceinline__ void argmax_combine(double& best, int64_t& bidx, double ob, int64_t oi) {
   // LAPACK idamax: largest |value|, first index wins ties; a NaN encountered first stays
   if (ob > best || (ob == best && oi < bidx)) { best = ob; bidx = oi; }
@@ -141,7 +126,7 @@ __device__ __forceinline__ size_t px_row_at(int buf, int rep, int cta, int kind,
 }
 
 __global__ void __launch_bounds__(DT) panel_coop_kernel(int64_t n, double* __restrict__ A, int64_t ld, int64_t c0, int kbi, int rpc,
-                                                         int64_t* __restrict__ ipiv, PanelScratch* __restrict__ ps, unsigned long long* __restrict__ xw) {
+                                                         int64_t* __restrict__ ipiv, int* __restrict__ info, unsigned long long* __restrict__ xw) {
   extern __shared__ double pa[];  // [kbi][rpc_pad]
   __shared__ double urow[NBI];
   __shared__ double smax[32];
@@ -224,13 +209,13 @@ __global__ void __launch_bounds__(DT) panel_coop_kernel(int64_t n, double* __res
     }
     __syncthreads();
     if (fault_s) {  // an exchange timed out: report through info and leave (every CTA times out on its own)
-      if (b == 0 && tid == 0) ps->info = -1;
+      if (b == 0 && tid == 0) *info = -1;
       break;
     }
     // (e) scale + rank-1 update of the rows below the diagonal
     const double pivval = urow[jj];
     if (pivval == 0.0) {
-      if (b == 0 && tid == 0 && ps->info == 0) ps->info = (int)(col + 1);
+      if (b == 0 && tid == 0 && *info == 0) *info = (int)(col + 1);
     } else {
       const double inv = 1.0 / pivval;
       for (int r = tid; r < nrows; r += DT) {
@@ -264,40 +249,12 @@ __global__ void __launch_bounds__(DT) swap_rows_kernel(double* __restrict__ A, i
   }
 }
 
-// X = L^{-1} X for the kb x ncols block at rows [r0, r0+kb), columns [c0, c0+ncols); L = unit lower triangle at (r0, r0)
-__global__ void __launch_bounds__(DT) trsm_kernel(double* __restrict__ A, int64_t ld, int64_t r0, int kb, int64_t c0, int64_t ncols) {
-  __shared__ double L[NBI][NBI + 1];
-  for (int t = threadIdx.x; t < kb * kb; t += blockDim.x) {
-    const int r = t % kb, c = t / kb;
-    L[r][c] = A[(r0 + c) * ld + r0 + r];
-  }
-  __syncthreads();
-  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= ncols) return;
-  double* col = A + (c0 + c) * ld + r0;
-  double x[NBI];
-#pragma unroll
-  for (int r = 0; r < NBI; ++r) x[r] = (r < kb) ? col[r] : 0.0;
-#pragma unroll
-  for (int r = 0; r < NBI; ++r) {
-    if (r < kb) {
-      double s = x[r];
-#pragma unroll
-      for (int q = 0; q < NBI; ++q)
-        if (q < r) s = fma(-L[r][q], x[q], s);
-      x[r] = s;
-    }
-  }
-#pragma unroll
-  for (int r = 0; r < NBI; ++r)
-    if (r < kb) col[r] = x[r];
-}
-
 // U12 = L11^{-1} A12 for a whole outer panel in ONE launch: a CTA owns U12_NCB columns of A12 and keeps its kbo x U12_NCB tile in
 // shared memory through all kbo / 32 block steps (warp-cooperative solve of the 32 x 32 unit-lower diagonal block — lanes are
 // rows, the solved entries travel by shuffle — then the rows below are updated with the solved block read back as 16-byte
 // broadcasts).  Replaces 31 dependent launches per outer step (16 solves of 32 rows + 15 updates), which had become pure launch
-// latency even when A12 is thousands of columns wide.  FP64 FMA-bound: kbo^2 / 2 per column.
+// latency even when A12 is thousands of columns wide.  FP64 FMA-bound: kbo^2 / 2 per column.  The inner panels use it too, with
+// kbo = kbi <= 32: one block step and no rows below.
 constexpr int U12_NCB = 16, U12_T = 256;
 __global__ void __launch_bounds__(U12_T, 2) u12_fused_kernel(double* __restrict__ A, int64_t ld, int64_t k0, int kbo, int64_t k1, int64_t rest) {
   extern __shared__ double xs[];                 // [U12_NCB][kbo] column-major tile of A12
@@ -365,11 +322,9 @@ __global__ void __launch_bounds__(U12_T, 2) u12_fused_kernel(double* __restrict_
 }
 
 // ------------------------------------------------------------------ C -= A * B on the FP64 tensor cores
-// A: M x K (lda), B: K x N (ldb), C: M x N (ldc), all column-major.  CTA = 4 warps, tile 128 (M) x 64 (N), each warp a
-// 32 x 64 sub-tile = 4 x 8 DMMA m8n8k4 accumulator fragments; K streamed in chunks of 8 through double-buffered shared
-// memory (rows padded by 4 doubles: fragment loads are bank-conflict free) with register prefetch of the next chunk.
-// 222 registers x 128 threads -> two CTAs per SM, so one CTA's C read-modify-write epilogue overlaps the other's MMAs.
-constexpr int GM_BM = 128, GM_BN = 64, GM_BK = 8, GM_PAD = 4, GM_T = 128, GM_STAGES = 4;
+// A: M x K (lda), B: K x N (ldb), C: M x N (ldc), all column-major.  Shared-memory rows are padded by 4 doubles, so the
+// fragment loads are bank-conflict free.
+constexpr int GM_BM = 128, GM_BN = 64, GM_BK = 8, GM_PAD = 4, GM_STAGES = 4;
 __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
@@ -384,17 +339,16 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 // K is streamed in chunks of 8 through a 4-stage cp.async ring: three chunks are always in flight underneath the MMAs of the
 // current one.  CTA = 8 warps (4 x 2), tile 128 (M) x 64 (N), each warp a 32 x 32 sub-tile = 4 x 4 DMMA m8n8k4 accumulator
-// fragments (64 registers): 119 registers per thread -> two CTAs = 16 warps per SM.  The FP64 tensor pipe of this part is fed
+// fragments (64 registers): 118 registers per thread -> two CTAs = 16 warps per SM.  The FP64 tensor pipe of this part is fed
 // by warps, not by tile size: fewer warps per SM (4 warps x (32 x 64) per CTA, or a persistent 128 x 128-tile kernel with ONE
 // 8-warp CTA per SM despite its better arithmetic intensity) factor the matrix more slowly.
 constexpr int G8_T = 256;
 constexpr int GM_SWZ = 16;  // tile columns per rasterisation group
-template <int MINB, int BK, int STAGES>
-__global__ void __launch_bounds__(G8_T, MINB) gemm_sub_w8_kernel(int64_t M, int64_t N, int K, const double* __restrict__ A, int64_t lda,
-                                                                  const double* __restrict__ B, int64_t ldb, double* __restrict__ C, int64_t ldc) {
+__global__ void __launch_bounds__(G8_T, 2) gemm_sub_w8_kernel(int64_t M, int64_t N, int K, const double* __restrict__ A, int64_t lda,
+                                                               const double* __restrict__ B, int64_t ldb, double* __restrict__ C, int64_t ldc) {
   extern __shared__ double gsm[];
-  double(*As)[BK][GM_BM + GM_PAD] = reinterpret_cast<double(*)[BK][GM_BM + GM_PAD]>(gsm);
-  double(*Bs)[BK][GM_BN + GM_PAD] = reinterpret_cast<double(*)[BK][GM_BN + GM_PAD]>(gsm + STAGES * BK * (GM_BM + GM_PAD));
+  double(*As)[GM_BK][GM_BM + GM_PAD] = reinterpret_cast<double(*)[GM_BK][GM_BM + GM_PAD]>(gsm);
+  double(*Bs)[GM_BK][GM_BN + GM_PAD] = reinterpret_cast<double(*)[GM_BK][GM_BN + GM_PAD]>(gsm + GM_STAGES * GM_BK * (GM_BM + GM_PAD));
   // Tile order: CTAs are dispatched with blockIdx.x fastest; taken literally every tile column (blockIdx.y) streams the whole
   // A panel (M x K: 132 MB at n = 32768, K = 512 — more than the 50 MB L2 keeps) from DRAM again, tens of GB of DRAM reads for
   // one trailing update.  Remapped in groups of GM_SWZ tile columns: consecutive CTAs
@@ -413,23 +367,23 @@ __global__ void __launch_bounds__(G8_T, MINB) gemm_sub_w8_kernel(int64_t M, int6
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = (warp & 3) * 32, wn = (warp >> 2) * 32;
   const int g = lane >> 2, t4 = lane & 3;
-  const int am = tid & 127, ak = tid >> 7;          // A staging: thread covers k = ak + 2 q, q = 0 .. BK/2-1
-  const int bk = tid & (BK - 1), bn = tid / BK;     // B staging: thread covers n = bn + (256/BK) q, q = 0 .. BK/4-1
+  const int am = tid & 127, ak = tid >> 7;             // A staging: thread covers k = ak + 2 q, q = 0 .. GM_BK/2-1
+  const int bk = tid & (GM_BK - 1), bn = tid / GM_BK;  // B staging: thread covers n = bn + (256/GM_BK) q, q = 0 .. GM_BK/4-1
   const bool m_ok = m0 + am < M;
   const double* a_src = A + (m_ok ? m0 + am : 0);
   auto issue_chunk = [&](int ch) {
-    const int st = ch % STAGES, kc = ch * BK;
+    const int st = ch % GM_STAGES, kc = ch * GM_BK;
 #pragma unroll
-    for (int q = 0; q < BK / 2; ++q) {
+    for (int q = 0; q < GM_BK / 2; ++q) {
       const int k = ak + 2 * q;
       const bool ok = m_ok && (kc + k < K);
       cp_async8(&As[st][k][am], a_src + (int64_t)(ok ? kc + k : 0) * lda, ok ? 8 : 0);
     }
 #pragma unroll
-    for (int q = 0; q < BK / 4; ++q) {
-      const int64_t nn = n0 + bn + (G8_T / BK) * q;
+    for (int q = 0; q < GM_BK / 4; ++q) {
+      const int64_t nn = n0 + bn + (G8_T / GM_BK) * q;
       const bool ok = (nn < N) && (kc + bk < K);
-      cp_async8(&Bs[st][bk][bn + (G8_T / BK) * q], B + (ok ? nn * ldb + kc + bk : 0), ok ? 8 : 0);
+      cp_async8(&Bs[st][bk][bn + (G8_T / GM_BK) * q], B + (ok ? nn * ldb + kc + bk : 0), ok ? 8 : 0);
     }
   };
   double acc[4][4][2];
@@ -437,20 +391,20 @@ __global__ void __launch_bounds__(G8_T, MINB) gemm_sub_w8_kernel(int64_t M, int6
   for (int a = 0; a < 4; ++a)
 #pragma unroll
     for (int b = 0; b < 4; ++b) acc[a][b][0] = acc[a][b][1] = 0.0;
-  const int nchunks = (K + BK - 1) / BK;
+  const int nchunks = (K + GM_BK - 1) / GM_BK;
 #pragma unroll
-  for (int s = 0; s < STAGES - 1; ++s) {
+  for (int s = 0; s < GM_STAGES - 1; ++s) {
     if (s < nchunks) issue_chunk(s);
     cp_async_commit();
   }
   for (int ch = 0; ch < nchunks; ++ch) {
-    cp_async_wait<STAGES - 2>();
+    cp_async_wait<GM_STAGES - 2>();
     __syncthreads();
-    if (ch + STAGES - 1 < nchunks) issue_chunk(ch + STAGES - 1);
+    if (ch + GM_STAGES - 1 < nchunks) issue_chunk(ch + GM_STAGES - 1);
     cp_async_commit();
-    const int st = ch % STAGES;
+    const int st = ch % GM_STAGES;
 #pragma unroll
-    for (int kk = 0; kk < BK; kk += 4) {
+    for (int kk = 0; kk < GM_BK; kk += 4) {
       double af[4], bf[4];
 #pragma unroll
       for (int a = 0; a < 4; ++a) af[a] = As[st][kk + t4][wm + a * 8 + g];
@@ -480,8 +434,8 @@ constexpr size_t GEMM_SMEM = sizeof(double) * GM_STAGES * GM_BK * ((GM_BM + GM_P
 int32_t gemm_sub(b200_ctx* ctx, int64_t M, int64_t N, int K, const double* A, int64_t lda, const double* B, int64_t ldb, double* C, int64_t ldc) {
   if (M <= 0 || N <= 0 || K <= 0) return B200_OK;
   dim3 grid((unsigned)((M + GM_BM - 1) / GM_BM), (unsigned)((N + GM_BN - 1) / GM_BN));
-  PLAUNCH(ctx, B200_KID_LU_GEMM, 2.0 * (double)M * (double)N * (double)K /* flops, not bytes */, (gemm_sub_w8_kernel<2, GM_BK, GM_STAGES>), grid, G8_T, GEMM_SMEM, M, N, K,
-          A, lda, B, ldb, C, ldc);
+  PLAUNCH(ctx, B200_KID_LU_GEMM, 2.0 * (double)M * (double)N * (double)K /* flops, not bytes */, gemm_sub_w8_kernel, grid, G8_T, GEMM_SMEM, M, N, K, A,
+          lda, B, ldb, C, ldc);
   return B200_OK;
 }
 
@@ -588,7 +542,7 @@ constexpr int QR_T = 1024;
 __global__ void __launch_bounds__(QR_T, 1) qrcp_kernel(int64_t n, double* __restrict__ A, int64_t ld, double* __restrict__ tau, int32_t* __restrict__ jpvt,
                                                         double* __restrict__ colnorm, int32_t* __restrict__ rank_out) {
   __shared__ double red_v[32];
-  __shared__ int red_i[32];
+  __shared__ int64_t red_i[32];
   __shared__ double s_a, s_b;
   __shared__ int s_p;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -607,26 +561,10 @@ __global__ void __launch_bounds__(QR_T, 1) qrcp_kernel(int64_t n, double* __rest
     }
     __syncthreads();
     double best = -1.0;
-    int bi = (int)k;
-    for (int64_t j = k + tid; j < n; j += QR_T) { const double v = colnorm[j]; if (v > best) { best = v; bi = (int)j; } }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double ov = __shfl_xor_sync(0xffffffffu, best, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-    }
-    if (lane == 0) { red_v[warp] = best; red_i[warp] = bi; }
-    __syncthreads();
-    if (warp == 0) {
-      best = red_v[lane]; bi = red_i[lane];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const double ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-      }
-      if (lane == 0) { s_p = bi; s_a = best; }
-    }
+    int64_t bi = k;
+    for (int64_t j = k + tid; j < n; j += QR_T) { const double v = colnorm[j]; if (v > best) { best = v; bi = j; } }
+    block_argmax(best, bi, red_v, red_i);  // result in warp 0
+    if (tid == 0) { s_p = (int)bi; s_a = best; }
     __syncthreads();
     const int64_t p = s_p;
     const double cn2 = s_a;
@@ -860,16 +798,15 @@ int32_t b200_dense_jac_fill(b200_problem* p, const double* u, double* J, int64_t
 int32_t b200_getrf(b200_ctx* ctx, int64_t n, double* A, int64_t ld, int64_t* ipiv, int32_t* info_host) {
   B200_DEVICE_GUARD(ctx);
   B200_REQUIRE(ctx, n > 0 && ld >= n, "getrf: bad dimensions");
-  static_assert(sizeof(PanelScratch) <= sizeof(double) * B200_RED_MAX_BLOCKS, "panel scratch must fit in d_partials");
-  PanelScratch* ps = reinterpret_cast<PanelScratch*>(ctx->d_partials + 2 * B200_RED_MAX_BLOCKS);
-  CUDA_TRY(ctx, cudaMemsetAsync(ps, 0, sizeof(PanelScratch), ctx->stream));
+  int* info = reinterpret_cast<int*>(ctx->d_partials + 2 * B200_RED_MAX_BLOCKS);  // first zero pivot (col + 1), -1: timeout
+  CUDA_TRY(ctx, cudaMemsetAsync(info, 0, sizeof(int), ctx->stream));
   if (!ctx->d_lu_xchg && cudaMalloc(&ctx->d_lu_xchg, sizeof(unsigned long long) * PX_WORDS) != cudaSuccess) {
     cudaGetLastError();
     return ctx->fail(B200_ERR_NOMEM, "getrf: exchange tables", __FILE__, __LINE__);
   }
   CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_lu_xchg, 0, sizeof(unsigned long long) * PX_WORDS, ctx->stream));  // epochs are column numbers: valid for one factorisation
   CUDA_TRY(ctx, cudaFuncSetAttribute(panel_coop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-  CUDA_TRY(ctx, cudaFuncSetAttribute((gemm_sub_w8_kernel<2, GM_BK, GM_STAGES>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
+  CUDA_TRY(ctx, cudaFuncSetAttribute(gemm_sub_w8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GEMM_SMEM));
   CUDA_TRY(ctx, cudaFuncSetAttribute(u12_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 512 * U12_NCB)));
   if (!ctx->aux_stream) {
     // highest priority: while the trailing update's CTAs drain and refill, the block scheduler hands freed SM slots to the
@@ -896,24 +833,15 @@ int32_t b200_getrf(b200_ctx* ctx, int64_t n, double* A, int64_t ld, int64_t* ipi
         int rpc = (int)((m + P - 1) / P);
         P = (int)((m + rpc - 1) / rpc);
         const size_t smem = sizeof(double) * (size_t)kbi * (size_t)(rpc | 1);
-        int kbi_ = kbi;
-        int64_t n_ = n, ld_ = ld, c0_ = c0;
-        double* A_ = A;
-        int64_t* ipiv_ = ipiv;
-        PanelScratch* ps_ = ps;
-        unsigned long long* xw_ = ctx->d_lu_xchg;
-        void* args[] = {&n_, &A_, &ld_, &c0_, &kbi_, &rpc, &ipiv_, &ps_, &xw_};
-        if (ctx->prof_on) ctx->prof_begin(B200_KID_LU_PANEL, 0.0);
-        CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)panel_coop_kernel, dim3(P), dim3(DT), args, smem, ctx->stream));
-        ctx->launches++;
-        if (ctx->prof_on) ctx->prof_end();
+        B200_TRY(coop_launch(ctx, B200_KID_LU_PANEL, 0.0, panel_coop_kernel, P, DT, smem, n, A, ld, c0, kbi, rpc, ipiv, info, ctx->d_lu_xchg));
         // the panel's interchanges applied to the other columns of the outer panel
         if (kbo - kbi > 0)
           PLAUNCH(ctx, B200_KID_LU_OTHER, 0.0, swap_rows_kernel, (int)((kbo - kbi + DT - 1) / DT), DT, 0, A, ld, c0, kbi, (const int64_t*)ipiv, k0, k1, c0, c1);
       }
       const int64_t rest = k1 - c1;  // rest of the outer panel: U = L11^{-1} A12 ; A22 -= L21 U
       if (rest > 0) {
-        PLAUNCH(ctx, B200_KID_LU_OTHER, 0.0, trsm_kernel, (int)((rest + DT - 1) / DT), DT, 0, A, ld, c0, kbi, c1, rest);
+        PLAUNCH(ctx, B200_KID_LU_OTHER, 0.0, u12_fused_kernel, (int)((rest + U12_NCB - 1) / U12_NCB), U12_T, sizeof(double) * kbi * U12_NCB, A, ld, c0,
+                kbi, c1, rest);
         B200_TRY(gemm_sub(ctx, n - c1, rest, kbi, A + c0 * ld + c1, ld, A + c1 * ld + c0, ld, A + c1 * ld + c1, ld));
       }
     }
@@ -923,18 +851,13 @@ int32_t b200_getrf(b200_ctx* ctx, int64_t n, double* A, int64_t ld, int64_t* ipi
   // outer block (the K of the trailing update): 512 for the big factorisations halves the C read-modify-write traffic
   // (n = 32768: 1.08 s -> 1.02 s; 768 buys nothing more), 256 below
   const int NBO = n >= 16384 ? 512 : NBO_DEFAULT;  // A/B knob for the outer block
-  const bool trace = getenv("B200_LU_TRACE") != nullptr;  // diagnostic: per-outer-step timeline of the main stream on stderr
-  std::vector<cudaEvent_t> tev;
-  auto mark = [&]() { if (trace) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s_main); tev.push_back(e); } };
   B200_TRY(factor_panel(0, (int)std::min<int64_t>(NBO, n)));
   for (int64_t k0 = 0; k0 < n; k0 += NBO) {
     const int kbo = (int)std::min<int64_t>(NBO, n - k0);
     const int64_t k1 = k0 + kbo;
-    mark();  // 0
     // ---- interchanges of this panel applied to the columns left and right of it
     if (n - kbo > 0)
       PLAUNCH(ctx, B200_KID_LU_OTHER, 0.0, swap_rows_kernel, (int)((n - kbo + DT - 1) / DT), DT, 0, A, ld, k0, kbo, (const int64_t*)ipiv, (int64_t)0, n, k0, k1);
-    mark();  // 0b: interchanges done
     const int64_t rest = n - k1;
     if (rest <= 0) break;
     // ---- U12 = L11^{-1} A12: one fused launch (column blocks of 16 stay in shared memory through all 16 block steps)
@@ -945,10 +868,8 @@ int32_t b200_getrf(b200_ctx* ctx, int64_t n, double* A, int64_t ld, int64_t* ipi
     // ---- trailing update on the FP64 tensor cores, with look-ahead: first the columns of the NEXT panel, whose
     //      factorisation (latency-bound, few SMs) then runs on a second stream underneath the rest of the GEMM.
     const int kbn = (int)std::min<int64_t>(NBO, rest);
-    mark();  // 1: swaps + U12 done
     B200_TRY(gemm_sub(ctx, rest, kbn, kbo, A + k0 * ld + k1, ld, A + k1 * ld + k0, ld, A + k1 * ld + k1, ld));
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_a, s_main));
-    mark();  // 2: look-ahead gemm done
     CUDA_TRY(ctx, cudaStreamWaitEvent(s_panel, ctx->ev_a, 0));
     ctx->stream = s_panel;
     int32_t st = factor_panel(k1, kbn);
@@ -957,25 +878,11 @@ int32_t b200_getrf(b200_ctx* ctx, int64_t n, double* A, int64_t ld, int64_t* ipi
     CUDA_TRY(ctx, cudaEventRecord(ctx->ev_b, s_panel));
     if (rest - kbn > 0)
       B200_TRY(gemm_sub(ctx, rest, rest - kbn, kbo, A + k0 * ld + k1, ld, A + (k1 + kbn) * ld + k0, ld, A + (k1 + kbn) * ld + k1, ld));
-    mark();  // 3: big gemm done
     CUDA_TRY(ctx, cudaStreamWaitEvent(s_main, ctx->ev_b, 0));
-    mark();  // 4: panel done
-  }
-  if (trace) {
-    cudaStreamSynchronize(s_main);
-    double seg[5] = {0, 0, 0, 0, 0};
-    fprintf(stderr, "[lu trace] step: swaps u12 lookahead biggemm panelwait (ms)\n");
-    for (size_t i = 0; i + 5 < tev.size(); i += 6) {
-      float t[5];
-      for (int j = 0; j < 5; ++j) { cudaEventElapsedTime(&t[j], tev[i + j], tev[i + j + 1]); seg[j] += t[j]; }
-      if ((i / 6) % 8 == 0) fprintf(stderr, "[lu trace] %3zu: %.3f %.3f %.3f %.3f %.3f\n", i / 6, t[0], t[1], t[2], t[3], t[4]);
-    }
-    fprintf(stderr, "[lu trace] totals: swaps %.1f u12 %.1f lookahead %.1f biggemm %.1f panelwait %.1f\n", seg[0], seg[1], seg[2], seg[3], seg[4]);
-    for (auto e : tev) cudaEventDestroy(e);
   }
   CHECK_LAUNCH(ctx);
   if (info_host) {
-    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_scalars + 16, &ps->info, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CUDA_TRY(ctx, cudaMemcpyAsync(ctx->h_scalars + 16, info, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
     *info_host = *reinterpret_cast<int*>(ctx->h_scalars + 16);
     if (*info_host < 0) return ctx->fail(B200_ERR_CUDA, "getrf: the panel's cross-CTA exchange timed out", __FILE__, __LINE__);

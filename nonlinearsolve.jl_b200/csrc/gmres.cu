@@ -1306,12 +1306,8 @@ int32_t gm_resident_step(b200_gmres* gm, const ResidentPlan& plan, int k) {
   RP.h = gm->d_h; RP.gsub = gm->d_gsub; RP.R = gm->d_R; RP.cs = gm->d_cs; RP.sn = gm->d_sn; RP.z = gm->d_z;
   RP.hraw = gm_hraw(gm, k);
   RP.st = gm->d_state;
-  void* args[] = {&RP};
-  if (ctx->prof_on) ctx->prof_begin(B200_KID_RESIDENT, resident_step_bytes(RP.passes, k, 8.0 * (double)gm->n));
-  CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)resident3g_arnoldi_kernel, dim3(RP.G), dim3(R3_THREADS), args, plan.smem, ctx->stream));
-  ctx->launches++;
-  if (ctx->prof_on) ctx->prof_end();
-  return B200_OK;
+  return coop_launch(ctx, B200_KID_RESIDENT, resident_step_bytes(RP.passes, k, 8.0 * (double)gm->n), resident3g_arnoldi_kernel, RP.G, R3_THREADS, plan.smem,
+                     RP);
 }
 }  // namespace
 

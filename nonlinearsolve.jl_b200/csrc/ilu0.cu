@@ -259,14 +259,7 @@ int32_t b200_ilu0_factor(b200_ilu0* ilu, const double* nzval, int32_t* info_host
   const int32_t none = INT_MAX;
   CUDA_TRY(ctx, cudaMemcpyAsync(ilu->d_info, &none, sizeof(int32_t), cudaMemcpyHostToDevice, ctx->stream));
   LAUNCH(ctx, ilu_gather_kernel, (int)((ilu->nnz + 255) / 256), 256, 0, ilu->nnz, (const int32_t*)ilu->d_map, nzval, ilu->d_lu);
-  IluParams P = params(ilu);
-  double* lu = ilu->d_lu;
-  int32_t* info = ilu->d_info;
-  void* args[] = {&P, &lu, &info};
-  if (ctx->prof_on) ctx->prof_begin(B200_KID_SPARSE, 0.0);
-  CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)ilu0_factor_kernel, dim3(ilu->grid), dim3(IL_THREADS), args, 0, ctx->stream));
-  ctx->launches++;
-  if (ctx->prof_on) ctx->prof_end();
+  B200_TRY(coop_launch(ctx, B200_KID_SPARSE, 0.0, ilu0_factor_kernel, ilu->grid, IL_THREADS, 0, params(ilu), ilu->d_lu, ilu->d_info));
   int32_t h = 0;
   CUDA_TRY(ctx, cudaMemcpyAsync(&h, ilu->d_info, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
@@ -279,14 +272,8 @@ int32_t b200_ilu0_solve(b200_ilu0* ilu, const double* b, double* x) {
   B200_DEVICE_GUARD(ilu ? ilu->ctx : nullptr);
   b200_ctx* ctx = ilu->ctx;
   B200_REQUIRE(ctx, ilu->factored, "ilu0_solve before ilu0_factor");
-  IluParams P = params(ilu);
-  const double* lu = ilu->d_lu;
-  void* args[] = {&P, &lu, &b, &x};
-  if (ctx->prof_on) ctx->prof_begin(B200_KID_SPARSE, 12.0 * (double)ilu->nnz + 3.0 * 8.0 * (double)ilu->n);
-  CUDA_TRY(ctx, cudaLaunchCooperativeKernel((const void*)ilu0_solve_kernel, dim3(ilu->grid), dim3(IL_THREADS), args, 0, ctx->stream));
-  ctx->launches++;
-  if (ctx->prof_on) ctx->prof_end();
-  return B200_OK;
+  return coop_launch(ctx, B200_KID_SPARSE, 12.0 * (double)ilu->nnz + 3.0 * 8.0 * (double)ilu->n, ilu0_solve_kernel, ilu->grid, IL_THREADS, 0, params(ilu),
+                     ilu->d_lu, b, x);
 }
 
 int32_t b200_ilu0_export(b200_ilu0* ilu, double* nzval_out) {
