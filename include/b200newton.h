@@ -112,8 +112,12 @@ enum { B200_QN_UPDATE_GOOD_BROYDEN = 0, B200_QN_UPDATE_BAD_BROYDEN = 1, B200_QN_
    geometric-multigrid V-cycle of the Brusselator Jacobian (the tutorial's AlgebraicMultigrid ruge_stuben / smoothed_aggregation) */
 /* ILU0: incomplete LU with zero fill of the assembled sparse Jacobian (b200_ilu0_*), refactorised with every fresh Jacobian;
    needs linsolve = SPARSE_GMRES and works on any problem with a pattern (built-in or a callback's jac_prototype) */
+/* AMG: one Ruge-Stueben algebraic-multigrid V-cycle of the assembled sparse Jacobian (b200_amg_*, default options): hierarchy
+   rebuilt at the first fresh Jacobian after create / reinit, values refreshed on the device with every later one; needs
+   linsolve = SPARSE_GMRES, any problem with a pattern */
 enum { B200_PRECOND_NONE = 0, B200_PRECOND_BLOCK_JACOBI_LEFT = 1, B200_PRECOND_BLOCK_JACOBI_RIGHT = 2,
-       B200_PRECOND_MULTIGRID_LEFT = 3, B200_PRECOND_MULTIGRID_RIGHT = 4, B200_PRECOND_ILU0_LEFT = 5, B200_PRECOND_ILU0_RIGHT = 6 };
+       B200_PRECOND_MULTIGRID_LEFT = 3, B200_PRECOND_MULTIGRID_RIGHT = 4, B200_PRECOND_ILU0_LEFT = 5, B200_PRECOND_ILU0_RIGHT = 6,
+       B200_PRECOND_AMG_LEFT = 7, B200_PRECOND_AMG_RIGHT = 8 };
 enum { B200_FORCING_NONE = 0, B200_FORCING_EW2 = 1 };
 /* termination modes (public.jl:300-407, termination_conditions.jl:243-372); `du` = f(u).  The three AbsNorm modes keep
    their round-1 values; Norm / Rel / RelNorm / Abs / RelNormSafe / RelNormSafeBest follow */
@@ -379,6 +383,45 @@ int32_t b200_ilu0_solve(b200_ilu0* ilu, const double* b_dev, double* x_dev);    
 int32_t b200_ilu0_export(b200_ilu0* ilu, double* nzval_out_dev);
 /* an operator applying U^-1 L^-1, for b200_gmres_set_precond; it borrows the handle (destroy the operator first) */
 int32_t b200_ilu0_linop(b200_ilu0* ilu, b200_linop** op);
+
+/* ---------------------------------------------------------------- algebraic multigrid preconditioner of an assembled sparse matrix
+ * Classical Ruge-Stueben AMG (the second `precs` of large_systems.md:244-316, with Jacobi smoothing; DESIGN.md §4h states the
+ * rules): classical strength (theta), the deterministic first-pass C/F splitting, direct interpolation, Galerkin coarse operators
+ * R A P with R = P', an explicit dense inverse of the coarsest level (at most 4096 unknowns).  The pattern (int32 CSR indices,
+ * n and every level's nnz < 2^31) is fixed at create.
+ *   setup(rebuild = 1): copies the values to the host, chooses the splitting and every pattern there, uploads them, then runs
+ *                       the device refresh;  setup(rebuild = 0): the splitting and patterns stay, the device recomputes every
+ *                       value (bit-reproducible; equal bits to a rebuild at the same values).
+ *   solve: one V(presweeps, postsweeps) cycle with damped Jacobi from x = 0, replayed as one CUDA graph; a fixed linear operator.
+ * info > 0: the 1-based level whose diagonal (or interpolation denominator) is zero or not finite, or whose dense LU met a zero
+ * pivot (coarsest level).  A hierarchy that ends above 4096 unknowns fails setup with B200_ERR_UNSUPPORTED. */
+typedef struct b200_amg b200_amg;
+typedef struct b200_amg_opts {
+  double theta;        /* strength threshold: 0.25 */
+  double omega;        /* Jacobi damping: 2/3 */
+  int32_t presweeps;   /* 1 */
+  int32_t postsweeps;  /* 1 */
+  int32_t max_levels;  /* 10 (the finest level counts) */
+  int32_t max_coarse;  /* 10: a level of at most this many unknowns is the coarsest */
+} b200_amg_opts;
+enum { B200_AMG_EXPORT_A = 0, B200_AMG_EXPORT_P = 1 };
+void b200_amg_opts_default(b200_amg_opts* opts);
+/* opts NULL: the defaults.  A row without a structural diagonal fails with B200_ERR_INVALID (the message names the row). */
+int32_t b200_amg_create(b200_ctx* ctx, int64_t n, const int64_t* colptr_host, const int64_t* rowval_host, int32_t index_base,
+                        const b200_amg_opts* opts, b200_amg** amg);
+int32_t b200_amg_destroy(b200_amg* amg);
+int32_t b200_amg_setup(b200_amg* amg, const double* nzval_dev, int32_t rebuild, int32_t* info_host);
+int32_t b200_amg_solve(b200_amg* amg, const double* b_dev, double* x_dev);  /* x = M^-1 b (x may alias b) */
+/* number of levels; the unknowns and nonzeros of the first `cap` of them */
+int32_t b200_amg_levels(b200_amg* amg, int32_t* nlev_host, int64_t* n_per_level_host, int64_t* nnz_per_level_host, int32_t cap);
+/* the CSR (0-based, int32 indices, columns ascending) of A_level or of P_level (n_level x n_level+1; not on the coarsest level);
+   rowptr holds n_level + 1 entries, col / val rowptr[n_level]; with col and val NULL only rowptr is written */
+int32_t b200_amg_export(b200_amg* amg, int32_t level, int32_t what, int32_t* rowptr_host, int32_t* col_host, double* val_host);
+/* an operator applying one V-cycle, for b200_gmres_set_precond; it borrows the handle (destroy the operator first) */
+int32_t b200_amg_linop(b200_amg* amg, b200_linop** op);
+/* the level-0 C/F splitting alone, on the host (no device): cf_out[i] = 1 for a C point, 0 for an F point */
+int32_t b200_amg_split(int64_t n, const int64_t* colptr_host, const int64_t* rowval_host, const double* nzval_host, int32_t index_base,
+                       double theta, int32_t* cf_out_host, int64_t* ncoarse_host);
 
 /* ---------------------------------------------------------------- Newton driver (a4, a7, a8, a9) */
 void b200_newton_opts_default(b200_newton_opts* opts);

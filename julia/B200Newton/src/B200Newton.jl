@@ -14,6 +14,7 @@
 module B200Newton
 
 using LinearAlgebra
+using SparseArrays: SparseMatrixCSC
 import SciMLBase
 import SciMLBase: ReturnCode, NLStats
 import CommonSolve
@@ -496,14 +497,76 @@ struct B200Multigrid <: B200Preconditioner end
 """`B200ILU0()`: incomplete LU with zero fill of the assembled sparse Jacobian.  It factors the concrete matrix, so it is offered
 on the whole-solve path only: `B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :ilu0_left | :ilu0_right)`."""
 struct B200ILU0 <: B200Preconditioner end
+"""`B200AMG()`: one Ruge-Stueben algebraic-multigrid V-cycle of the assembled sparse Jacobian (Jacobi smoothing).  It coarsens
+the concrete matrix, so it is offered on the whole-solve path only: `B200NewtonKrylov(; linsolve = :sparse_gmres,
+precs = :amg_left | :amg_right)`; `AMGHierarchy` is the stand-alone handle."""
+struct B200AMG <: B200Preconditioner end
 precond_kind(::B200BlockJacobi) = Int32(1)      # B200_PRECOND_BLOCK_JACOBI_LEFT (LEFT / RIGHT of a family name the same operator)
 precond_kind(::B200Multigrid) = Int32(3)        # B200_PRECOND_MULTIGRID_LEFT
 precond_op(::B200ILU0, ::Problem, ::B200Vector) = throw(ArgumentError(
     "B200ILU0 needs the concrete sparse Jacobian: use B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :ilu0_left) (or :ilu0_right)"))
+precond_op(::B200AMG, ::Problem, ::B200Vector) = throw(ArgumentError(
+    "B200AMG needs the concrete sparse Jacobian: use B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :amg_left) (or :amg_right)"))
 function precond_op(P::B200Preconditioner, prob::Problem, u::B200Vector)
     op = Ref{Ptr{Cvoid}}(C_NULL)
     check(prob.ctx.handle, @ccall libb200.b200_linop_precond(prob.handle::Ptr{Cvoid}, u.ptr::Ptr{Float64}, precond_kind(P)::Int32, op::Ref{Ptr{Cvoid}})::Int32)
     return op[]
+end
+
+# ------------------------------------------------------------------ algebraic multigrid of an assembled CSC matrix (b200_amg_*)
+struct AmgOpts
+    theta::Float64
+    omega::Float64
+    presweeps::Int32
+    postsweeps::Int32
+    max_levels::Int32
+    max_coarse::Int32
+end
+function default_amg_opts()
+    o = Ref{AmgOpts}()
+    @ccall libb200.b200_amg_opts_default(o::Ref{AmgOpts})::Cvoid
+    return o[]
+end
+
+"""`AMGHierarchy(ctx, A::SparseMatrixCSC; opts = default_amg_opts())`: the device Ruge-Stueben hierarchy of A's pattern.
+`setup!(h, nzval; rebuild = true)` returns 0 or the 1-based level of a zero diagonal / pivot; `ldiv!(x, h, b)` applies one
+V-cycle; `amg_levels(h)` the unknowns and nonzeros per level."""
+mutable struct AMGHierarchy
+    ctx::Context
+    handle::Ptr{Cvoid}
+    n::Int
+    function AMGHierarchy(ctx::Context, A::SparseMatrixCSC; opts::AmgOpts = default_amg_opts())
+        n = size(A, 1)
+        h = Ref{Ptr{Cvoid}}(C_NULL)
+        colptr, rowval = Vector{Int64}(A.colptr), Vector{Int64}(A.rowval)
+        check(ctx.handle, @ccall libb200.b200_amg_create(ctx.handle::Ctx, n::Int64, colptr::Ptr{Int64}, rowval::Ptr{Int64}, 1::Int32, Ref(opts)::Ref{AmgOpts},
+                                                         h::Ref{Ptr{Cvoid}})::Int32)
+        H = new(ctx, h[], n)
+        finalizer(x -> (@ccall libb200.b200_amg_destroy(x.handle::Ptr{Cvoid})::Int32), H)
+        return H
+    end
+end
+function setup!(H::AMGHierarchy, nzval::B200Vector; rebuild::Bool = true)
+    info = Ref{Int32}(0)
+    check(H.ctx.handle, @ccall libb200.b200_amg_setup(H.handle::Ptr{Cvoid}, nzval.ptr::Ptr{Float64}, Int32(rebuild)::Int32, info::Ref{Int32})::Int32)
+    return Int(info[])
+end
+LinearAlgebra.ldiv!(x::B200Vector, H::AMGHierarchy, b::B200Vector) =
+    (check(H.ctx.handle, @ccall libb200.b200_amg_solve(H.handle::Ptr{Cvoid}, b.ptr::Ptr{Float64}, x.ptr::Ptr{Float64})::Int32); x)
+function amg_levels(H::AMGHierarchy)
+    nl = Ref{Int32}(0)
+    ns, nz = zeros(Int64, 64), zeros(Int64, 64)
+    check(H.ctx.handle, @ccall libb200.b200_amg_levels(H.handle::Ptr{Cvoid}, nl::Ref{Int32}, ns::Ptr{Int64}, nz::Ptr{Int64}, 64::Int32)::Int32)
+    return ns[1:nl[]], nz[1:nl[]]
+end
+"""`amg_split(A::SparseMatrixCSC; theta = 0.25)`: the level-0 C/F splitting on the host (true at C points), no device."""
+function amg_split(A::SparseMatrixCSC; theta::Real = 0.25)
+    n = size(A, 1)
+    cf, nc = zeros(Int32, n), Ref{Int64}(0)
+    st = @ccall libb200.b200_amg_split(n::Int64, Vector{Int64}(A.colptr)::Ptr{Int64}, Vector{Int64}(A.rowval)::Ptr{Int64}, Vector{Float64}(A.nzval)::Ptr{Float64},
+                                       1::Int32, Float64(theta)::Float64, cf::Ptr{Int32}, nc::Ref{Int64})::Int32
+    st == 0 || throw(B200Error(st, "b200_amg_split failed"))
+    return cf .== 1
 end
 
 # ------------------------------------------------------------------ whole-solve fast path
@@ -541,7 +604,8 @@ const _DESCENT = (newton = 0, pseudo_transient = 1, levenberg_marquardt = 2, bro
 const _QN_INIT = (identity = 0, true_jacobian = 1, low_rank = 2)
 const _QN_UPDATE = (good_broyden = 0, bad_broyden = 1, klement = 2)
 const _TR_SCHEMES = (simple = 0, nlsolve = 1, nocedal_wright = 2, hei = 3, yuan = 4, fan = 5, bastin = 6)
-const _PRECS = (none = 0, block_jacobi_left = 1, block_jacobi_right = 2, multigrid_left = 3, multigrid_right = 4, ilu0_left = 5, ilu0_right = 6)
+const _PRECS = (none = 0, block_jacobi_left = 1, block_jacobi_right = 2, multigrid_left = 3, multigrid_right = 4, ilu0_left = 5, ilu0_right = 6, amg_left = 7,
+    amg_right = 8)
 const _TERMINATION = (abs_norm_safe_best = 0, abs_norm = 1, abs_norm_safe = 2, norm = 3, rel = 4, rel_norm = 5, abs = 6,
     rel_norm_safe = 7, rel_norm_safe_best = 8)
 
@@ -674,7 +738,7 @@ function SciMLBase.__solve(ens::SciMLBase.AbstractEnsembleProblem, alg::B200Newt
     return SciMLBase.EnsembleSolution(sols, time() - t0, converged)
 end
 
-export Context, B200Vector, brusselator, brusselator_function, initial_condition, B200GMRES, B200BlockJacobi, B200Multigrid, B200ILU0,
+export Context, B200Vector, brusselator, brusselator_function, initial_condition, B200GMRES, B200BlockJacobi, B200Multigrid, B200ILU0, B200AMG, AMGHierarchy, setup!, amg_levels, amg_split,
     B200NewtonKrylov, EnsembleB200, nccl_unique_id, device_count
 
 end # module

@@ -427,6 +427,22 @@ class ILU0:
         return abi.PRECOND_ILU0_LEFT if self.side == "left" else abi.PRECOND_ILU0_RIGHT
 
 
+class RugeStubenAMG:
+    """Preconditioner for `KrylovJL_GMRES(precs = ...)` on the concrete sparse Jacobian: one classical Ruge-Stueben algebraic
+    multigrid V-cycle with damped Jacobi smoothing — the tutorial's `AlgebraicMultigrid.aspreconditioner(ruge_stuben(W))` with
+    Jacobi smoothers (docs/src/tutorials/large_systems.md:244-316), default options (theta 0.25, omega 2/3, V(1,1)).  The
+    splitting is chosen at the first fresh Jacobian of a solve; later Jacobians refresh every value on the device.  Needs
+    `concrete_jac = True` or a sparse prototype, and serves any problem with a pattern, including `jac_prototype`."""
+
+    def __init__(self, side="left"):
+        assert side in ("left", "right")
+        self.side = side
+
+    @property
+    def code(self):
+        return abi.PRECOND_AMG_LEFT if self.side == "left" else abi.PRECOND_AMG_RIGHT
+
+
 class LUFactorization:
     needs_concrete_A = True
 
@@ -506,6 +522,82 @@ class SparseILU0:
         op = C.c_void_p()
         check(self.ctx.handle, lib().b200_ilu0_linop(self._h, C.byref(op)))
         return op
+
+
+class SparseAMG:
+    """Direct handle on the device Ruge-Stueben hierarchy of a CSC pattern (colptr, rowval host arrays, 1-based by default).
+    Options: theta, omega, presweeps, postsweeps, max_levels, max_coarse (b200_amg_opts).  `setup(nzval, rebuild=True)` returns
+    0 or the 1-based level of a zero diagonal / pivot (rebuild=False keeps the splitting and recomputes the values), `solve(b)`
+    applies one V-cycle, `levels()` returns the unknowns and nonzeros per level, `level(l)` the CSR arrays of A_l and P_l."""
+
+    def __init__(self, ctx, n, colptr, rowval, index_base=1, **opts):
+        self.ctx, self.n = ctx, n
+        colptr = np.ascontiguousarray(colptr, dtype=np.int64)
+        rowval = np.ascontiguousarray(rowval, dtype=np.int64)
+        o = abi.AmgOpts()
+        lib().b200_amg_opts_default(C.byref(o))
+        for k, v in opts.items():
+            assert k in dict(abi.AmgOpts._fields_), k
+            setattr(o, k, v)
+        self.opts = o
+        self._h = C.c_void_p()
+        check(ctx.handle, lib().b200_amg_create(ctx.handle, n, colptr.ctypes.data_as(C.c_void_p), rowval.ctypes.data_as(C.c_void_p), index_base,
+                                                C.byref(o), C.byref(self._h)))
+        self._fin = ctx._adopt(weakref.finalize(self, lib().b200_amg_destroy, self._h))
+
+    def setup(self, nzval, rebuild=True):
+        info = C.c_int32(0)
+        check(self.ctx.handle, lib().b200_amg_setup(self._h, nzval.ptr, int(bool(rebuild)), C.byref(info)))
+        return info.value
+
+    def solve(self, b, x=None):
+        x = x or self.ctx.zeros(self.n)
+        check(self.ctx.handle, lib().b200_amg_solve(self._h, b.ptr, x.ptr))
+        return x
+
+    def levels(self):
+        cap = 64
+        nl = C.c_int32(0)
+        ns, nz = np.zeros(cap, dtype=np.int64), np.zeros(cap, dtype=np.int64)
+        check(self.ctx.handle, lib().b200_amg_levels(self._h, C.byref(nl), ns.ctypes.data_as(C.c_void_p), nz.ctypes.data_as(C.c_void_p), cap))
+        return ns[:nl.value].tolist(), nz[:nl.value].tolist()
+
+    def _export(self, level, what, nrows):
+        rowptr = np.zeros(nrows + 1, dtype=np.int32)
+        check(self.ctx.handle, lib().b200_amg_export(self._h, level, what, rowptr.ctypes.data_as(C.c_void_p), None, None))
+        col = np.zeros(int(rowptr[-1]), dtype=np.int32)
+        val = np.zeros(int(rowptr[-1]), dtype=np.float64)
+        check(self.ctx.handle, lib().b200_amg_export(self._h, level, what, rowptr.ctypes.data_as(C.c_void_p), col.ctypes.data_as(C.c_void_p),
+                                                     val.ctypes.data_as(C.c_void_p)))
+        return val, col, rowptr
+
+    def level(self, l):
+        """{"A": (data, indices, indptr), "P": ... or None on the coarsest level}: `scipy.sparse.csr_matrix(level["A"])` builds A_l."""
+        ns, _ = self.levels()
+        out = {"A": self._export(l, abi.AMG_EXPORT_A, ns[l]), "P": None}
+        if l + 1 < len(ns):
+            out["P"] = self._export(l, abi.AMG_EXPORT_P, ns[l])
+        return out
+
+    def linop(self):
+        """A borrowed-by-GMRES operator handle applying one V-cycle (destroy it with b200_linop_destroy before this handle)."""
+        op = C.c_void_p()
+        check(self.ctx.handle, lib().b200_amg_linop(self._h, C.byref(op)))
+        return op
+
+
+def amg_split(n, colptr, rowval, nzval, index_base=1, theta=0.25):
+    """The level-0 Ruge-Stueben C/F splitting on the host (no device): (boolean array, True at C points; number of C points)."""
+    colptr = np.ascontiguousarray(colptr, dtype=np.int64)
+    rowval = np.ascontiguousarray(rowval, dtype=np.int64)
+    nzval = np.ascontiguousarray(nzval, dtype=np.float64)
+    cf = np.zeros(n, dtype=np.int32)
+    nc = C.c_int64()
+    st = lib().b200_amg_split(n, colptr.ctypes.data_as(C.c_void_p), rowval.ctypes.data_as(C.c_void_p), nzval.ctypes.data_as(C.c_void_p), index_base,
+                              theta, cf.ctypes.data_as(C.c_void_p), C.byref(nc))
+    if st != abi.OK:
+        raise abi.B200Error(st, "b200_amg_split failed")
+    return cf.astype(bool), nc.value
 
 
 class AutoForwardDiff:

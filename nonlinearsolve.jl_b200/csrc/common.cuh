@@ -259,9 +259,10 @@ struct b200_linop {
   int32_t owns_mg;
   int64_t *csr_rowptr, *csr_col, *csr_map;  // LINOP_CSC: row view of the pattern (owned), built once so that y = A x is a deterministic gather
   b200_ilu0* ilu;  // LINOP_ILU0: the factors (borrowed)
+  b200_amg* amg;   // LINOP_AMG: the hierarchy (borrowed)
 };
 enum { LINOP_PROBLEM = 0, LINOP_CSC = 1, LINOP_DENSE = 2, LINOP_CALLBACK = 3, LINOP_SPARSE_JAC = 4, LINOP_BLOCK_JACOBI = 5, LINOP_MULTIGRID = 6,
-       LINOP_ILU0 = 7 };
+       LINOP_ILU0 = 7, LINOP_AMG = 8 };
 
 // internal (non-ABI) helpers implemented across the .cu files
 // Host callbacks run user device code on streams the library knows nothing about (its own stream is non-blocking): drain
@@ -273,6 +274,11 @@ static inline int32_t b200i_sync_for_callback(b200_ctx* ctx) {
   return B200_OK;
 }
 int32_t b200i_linop_apply(b200_linop* op, const double* x, double* y);
+// row view of a CSC pattern (ilu0.cu): int32 CSR with columns ascending, map = CSR position -> caller's CSC position, diag =
+// the position of each row's diagonal (-1: none).  Empty string on success, else the message ("<who>: ..."; a missing
+// diagonal, when required, names the row).
+std::string b200i_csr_of_csc(const char* who, int64_t n, const int64_t* colptr, const int64_t* rowval, int32_t base, bool require_diag,
+                             std::vector<int32_t>& rowptr, std::vector<int32_t>& col, std::vector<int32_t>& map, std::vector<int32_t>& diag);
 // geometric multigrid preconditioner of the built-in Brusselator Jacobian (mg.cu)
 int32_t b200i_mg_create(b200_problem* prob, b200_mg** out);
 int32_t b200i_mg_destroy(b200_mg* mg);

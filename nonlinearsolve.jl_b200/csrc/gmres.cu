@@ -1203,6 +1203,8 @@ static int32_t linop_apply_unshifted(b200_linop* op, const double* x, double* y)
       return b200i_mg_apply(op->mg, x, y);
     case LINOP_ILU0:
       return b200_ilu0_solve(op->ilu, x, y);
+    case LINOP_AMG:
+      return b200_amg_solve(op->amg, x, y);
     case LINOP_BLOCK_JACOBI: {
       const int64_t NC = op->n / 2;
       const double lapdiag = -(op->prob->kind == B200_PROB_BRUSS3D ? 6.0 : 4.0) * op->prob->a;
@@ -1505,6 +1507,8 @@ int32_t b200_linop_precond(b200_problem* prob, const double* u, int32_t kind, b2
   if (kind == B200_PRECOND_BLOCK_JACOBI_LEFT || kind == B200_PRECOND_BLOCK_JACOBI_RIGHT) return b200_linop_block_jacobi(prob, u, out);
   B200_REQUIRE(ctx, kind != B200_PRECOND_ILU0_LEFT && kind != B200_PRECOND_ILU0_RIGHT,
                "linop_precond: ILU0 factors the assembled sparse Jacobian, not a problem: use b200_ilu0_create / b200_ilu0_factor / b200_ilu0_linop");
+  B200_REQUIRE(ctx, kind != B200_PRECOND_AMG_LEFT && kind != B200_PRECOND_AMG_RIGHT,
+               "linop_precond: AMG coarsens the assembled sparse Jacobian, not a problem: use b200_amg_create / b200_amg_setup / b200_amg_linop");
   B200_REQUIRE(ctx, kind == B200_PRECOND_MULTIGRID_LEFT || kind == B200_PRECOND_MULTIGRID_RIGHT, "linop_precond: unknown preconditioner kind");
   b200_mg* mg = nullptr;
   B200_TRY(b200i_mg_create(prob, &mg));

@@ -164,6 +164,45 @@ IluParams params(const b200_ilu0* ilu) {
 }
 }  // namespace
 
+std::string b200i_csr_of_csc(const char* who, int64_t n, const int64_t* colptr, const int64_t* rowval, int32_t base, bool require_diag,
+                             std::vector<int32_t>& rowptr, std::vector<int32_t>& col, std::vector<int32_t>& map, std::vector<int32_t>& diag) {
+  const int64_t nnz = colptr[n] - colptr[0];
+  char msg[200];
+  // CSR view: walking the columns in order leaves every row's column indices ascending
+  rowptr.assign(n + 1, 0); col.assign(nnz, 0); map.assign(nnz, 0); diag.assign(n, -1);
+  for (int64_t c = 0; c < n; ++c) {
+    if (colptr[c + 1] < colptr[c]) { snprintf(msg, sizeof(msg), "%s: colptr must be non-decreasing", who); return msg; }
+    for (int64_t p = colptr[c] - base; p < colptr[c + 1] - base; ++p) {
+      const int64_t r = rowval[p] - base;
+      if (r < 0 || r >= n) { snprintf(msg, sizeof(msg), "%s: row index out of range", who); return msg; }
+      rowptr[r + 1]++;
+    }
+  }
+  for (int64_t r = 0; r < n; ++r) rowptr[r + 1] += rowptr[r];
+  {
+    std::vector<int32_t> fill(rowptr.begin(), rowptr.end() - 1);
+    for (int64_t c = 0; c < n; ++c)
+      for (int64_t p = colptr[c] - base; p < colptr[c + 1] - base; ++p) {
+        const int32_t q = fill[rowval[p] - base]++;
+        col[q] = (int32_t)c; map[q] = (int32_t)p;
+      }
+  }
+  for (int64_t r = 0; r < n; ++r) {
+    for (int32_t q = rowptr[r]; q < rowptr[r + 1]; ++q) {
+      if (q > rowptr[r] && col[q] == col[q - 1]) {
+        snprintf(msg, sizeof(msg), "%s: duplicate entry (%lld, %lld) in the pattern", who, (long long)(r + base), (long long)(col[q] + base));
+        return msg;
+      }
+      if (col[q] == r) diag[r] = q;
+    }
+    if (require_diag && diag[r] < 0) {
+      snprintf(msg, sizeof(msg), "%s: row %lld (index base %d) has no structural diagonal entry", who, (long long)(r + base), (int)base);
+      return msg;
+    }
+  }
+  return std::string();
+}
+
 extern "C" {
 int32_t b200_ilu0_destroy(b200_ilu0* ilu) {
   if (!ilu) return B200_OK;
@@ -182,40 +221,9 @@ int32_t b200_ilu0_create(b200_ctx* ctx, int64_t n, const int64_t* colptr, const 
   const int64_t nnz = colptr[n] - colptr[0];
   B200_REQUIRE(ctx, colptr[0] == base && nnz >= 0, "ilu0_create: colptr must start at the index base");
   B200_REQUIRE(ctx, n < INT32_MAX && nnz < INT32_MAX, "ilu0_create: n and nnz must be below 2^31 (int32 CSR indices)");
-  // CSR view: walking the columns in order leaves every row's column indices ascending
-  std::vector<int32_t> rowptr(n + 1, 0), col(nnz), map(nnz), diag(n, -1);
-  for (int64_t c = 0; c < n; ++c) {
-    B200_REQUIRE(ctx, colptr[c + 1] >= colptr[c], "ilu0_create: colptr must be non-decreasing");
-    for (int64_t p = colptr[c] - base; p < colptr[c + 1] - base; ++p) {
-      const int64_t r = rowval[p] - base;
-      if (r < 0 || r >= n) return ctx->fail(B200_ERR_INVALID, "ilu0_create: row index out of range", __FILE__, __LINE__);
-      rowptr[r + 1]++;
-    }
-  }
-  for (int64_t r = 0; r < n; ++r) rowptr[r + 1] += rowptr[r];
-  {
-    std::vector<int32_t> fill(rowptr.begin(), rowptr.end() - 1);
-    for (int64_t c = 0; c < n; ++c)
-      for (int64_t p = colptr[c] - base; p < colptr[c + 1] - base; ++p) {
-        const int32_t q = fill[rowval[p] - base]++;
-        col[q] = (int32_t)c; map[q] = (int32_t)p;
-      }
-  }
-  for (int64_t r = 0; r < n; ++r) {
-    for (int32_t q = rowptr[r]; q < rowptr[r + 1]; ++q) {
-      if (q > rowptr[r] && col[q] == col[q - 1]) {
-        char msg[160];
-        snprintf(msg, sizeof(msg), "ilu0_create: duplicate entry (%lld, %lld) in the pattern", (long long)(r + base), (long long)(col[q] + base));
-        return ctx->fail(B200_ERR_INVALID, msg, __FILE__, __LINE__);
-      }
-      if (col[q] == r) diag[r] = q;
-    }
-    if (diag[r] < 0) {
-      char msg[160];
-      snprintf(msg, sizeof(msg), "ilu0_create: row %lld (index base %d) has no structural diagonal entry", (long long)(r + base), (int)base);
-      return ctx->fail(B200_ERR_INVALID, msg, __FILE__, __LINE__);
-    }
-  }
+  std::vector<int32_t> rowptr, col, map, diag;
+  const std::string err = b200i_csr_of_csc("ilu0_create", n, colptr, rowval, base, true, rowptr, col, map, diag);
+  if (!err.empty()) return ctx->fail(B200_ERR_INVALID, err.c_str(), __FILE__, __LINE__);
   std::vector<int32_t> lrows, lptr, urows, uptr;
   level_sets(n, rowptr, col, diag, true, lrows, lptr);
   level_sets(n, rowptr, col, diag, false, urows, uptr);

@@ -64,6 +64,9 @@ struct b200_newton {
   b200_sparse_lu* slu;  // LINSOLVE_SPARSE_LU: band factorisation of the assembled Jacobian
   b200_ilu0* ilu;       // PRECOND_ILU0_*: incomplete LU of the assembled Jacobian, refactorised with every fresh J
   int32_t ilu_info;     // its last factorisation: 0, or the 1-based row of a zero / non-finite pivot
+  b200_amg* amg;        // PRECOND_AMG_*: Ruge-Stueben hierarchy of the assembled Jacobian
+  int32_t amg_info;     // its last setup: 0, or the 1-based level of a zero diagonal / pivot
+  int32_t amg_built;    // a hierarchy exists for this solve: later fresh Jacobians refresh its values (reset by reinit)
   // LevenbergMarquardt: J'J + lambda D'D (factored in place), the running diagonal D'D, velocity / acceleration, previous velocity, J' f
   double *lmA, *lm_dtd, *lm_v, *lm_a, *lm_vold, *lm_rhs;
   double lm_lambda, lm_lambda_factor, lm_norm_v_old, lm_loss_old;
@@ -229,11 +232,13 @@ int32_t b200_newton_destroy(b200_newton* nw) {
   if (nw->sj) b200_sparse_jac_destroy(nw->sj);
   if (nw->slu) b200_sparse_lu_destroy(nw->slu);
   if (nw->ilu) b200_ilu0_destroy(nw->ilu);
+  if (nw->amg) b200_amg_destroy(nw->amg);
   delete nw;
   return B200_OK;
 }
 
 static bool ilu0_precond(const b200_newton_opts& o) { return o.precond == B200_PRECOND_ILU0_LEFT || o.precond == B200_PRECOND_ILU0_RIGHT; }
+static bool amg_precond(const b200_newton_opts& o) { return o.precond == B200_PRECOND_AMG_LEFT || o.precond == B200_PRECOND_AMG_RIGHT; }
 
 // the buffers and sub-solvers b200_newton_create builds for the options; on failure the caller destroys the partial driver
 static int32_t newton_setup(b200_newton* nw) {
@@ -294,6 +299,7 @@ static int32_t newton_setup(b200_newton* nw) {
     // sparse direct route (linsolve = nothing on a sparse prototype): symbolic phase once, like LinearSolve's cache
     if (o.linsolve == B200_LINSOLVE_SPARSE_LU) B200_TRY(b200_sparse_lu_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->slu));
     if (ilu0_precond(o)) B200_TRY(b200_ilu0_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->ilu));
+    if (amg_precond(o)) B200_TRY(b200_amg_create(ctx, n, colptr.data(), rowval.data(), 1, nullptr, &nw->amg));
     nw->op.kind = LINOP_SPARSE_JAC; nw->op.sj = nw->sj; nw->op.nzval = nw->nzval;
   } else {
     return ctx->fail(B200_ERR_INVALID, "unknown linsolve kind", __FILE__, __LINE__);
@@ -319,8 +325,14 @@ int32_t b200_newton_create(b200_problem* prob, const b200_newton_opts* opts, b20
                           (opts->qn_update_rule == B200_QN_UPDATE_KLEMENT && opts->qn_init_jacobian == B200_QN_INIT_IDENTITY))),
                "newton_create: descent must be Newton, PseudoTransient (without a trust region), LevenbergMarquardt (dense concrete Jacobian, its own trust region) or "
                "Broyden (no globalisation, n <= 65535, init_jacobian = true_jacobian needs the dense LU)");
-  B200_REQUIRE(ctx, opts->precond >= B200_PRECOND_NONE && opts->precond <= B200_PRECOND_ILU0_RIGHT, "newton_create: unknown preconditioner");
-  if (ilu0_precond(*opts)) {
+  B200_REQUIRE(ctx, opts->precond >= B200_PRECOND_NONE && opts->precond <= B200_PRECOND_AMG_RIGHT, "newton_create: unknown preconditioner");
+  if (amg_precond(*opts)) {
+    // AMG coarsens the assembled sparse Jacobian (any pattern); PseudoTransient's shift changes every step, as for ILU0
+    B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_SPARSE_GMRES,
+                 "newton_create: the AMG preconditioner coarsens the assembled sparse Jacobian: use concrete_jac = true (linsolve B200_LINSOLVE_SPARSE_GMRES)");
+    if (opts->descent == B200_DESCENT_PSEUDO_TRANSIENT)
+      return ctx->fail(B200_ERR_UNSUPPORTED, "newton_create: PseudoTransient with the AMG preconditioner is not offered (use block-Jacobi, multigrid or no preconditioner)", __FILE__, __LINE__);
+  } else if (ilu0_precond(*opts)) {
     // ILU(0) factors the assembled sparse Jacobian, so any problem with a pattern qualifies; the SER shift of PseudoTransient
     // changes every step and would need a refactorisation every step, as on the sparse direct route
     B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_SPARSE_GMRES,
@@ -352,6 +364,7 @@ int32_t b200_newton_reinit(b200_newton* nw, const double* u0_dev) {
   const int64_t n = nw->n;
   const b200_newton_opts& o = nw->o;
   if (u0_dev != nw->u) CUDA_TRY(ctx, cudaMemcpyAsync(nw->u, u0_dev, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
+  nw->amg_built = 0;  // the first fresh Jacobian of this solve rebuilds the AMG hierarchy
   CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double) * 4, ctx->stream));
   B200_TRY(b200i_residual_norm(nw->prob, nw->u, nw->fu, ctx->d_scalars));  // evaluate_f(prob,u): nf is NOT bumped (solve.jl:194)
   CUDA_TRY(ctx, cudaMemsetAsync(nw->du, 0, sizeof(double) * n, ctx->stream));  // descent caches start with a defined du
@@ -760,6 +773,10 @@ static int32_t refresh_jacobian(b200_newton* nw, bool* fresh) {
   B200_TRY(b200_sparse_jac_fill(nw->sj, nw->u, nw->nzval));
   // precs(A, p) on the new A; not an NLStats factorisation (LinearSolve's Krylov route counts none)
   if (nw->ilu) B200_TRY(b200_ilu0_factor(nw->ilu, nw->nzval, &nw->ilu_info));
+  if (nw->amg) {  // the splitting is chosen once per solve; later Jacobians refresh the values on the device
+    B200_TRY(b200_amg_setup(nw->amg, nw->nzval, !nw->amg_built, &nw->amg_info));
+    nw->amg_built = nw->amg_info == 0;
+  }
   return B200_OK;
 }
 
@@ -844,6 +861,7 @@ static int32_t linear_solve(b200_newton* nw, bool fresh, bool* ok, b200_gmres_st
     // `linu` aliases the du buffer: it is the initial guess only when warm_start is requested
     if (o.gmres.warm_start) CUDA_TRY(ctx, cudaMemcpyAsync(nw->xlin, nw->du, sizeof(double) * n, cudaMemcpyDeviceToDevice, ctx->stream));
     if (nw->ilu && nw->ilu_info != 0) { *ok = false; return B200_OK; }  // zero pivot: a failed solve, retried with a fresh Jacobian
+    if (nw->amg && nw->amg_info != 0) { *ok = false; return B200_OK; }  // zero diagonal or pivot: likewise
     if (o.precond != B200_PRECOND_NONE) {  // precs(A, p): rebuilt from the current iterate, like update_A! does for Pl / Pr
       memset(&nw->prec, 0, sizeof(nw->prec));
       nw->prec.ctx = ctx; nw->prec.n = n; nw->prec.prob = nw->prob; nw->prec.u = nw->u;
@@ -852,10 +870,13 @@ static int32_t linear_solve(b200_newton* nw, bool fresh, bool* ok, b200_gmres_st
         if (fresh) B200_TRY(b200i_mg_setup(nw->mg, nw->u));  // coarse operators follow the linearisation point
       } else if (nw->ilu) {
         nw->prec.kind = LINOP_ILU0; nw->prec.ilu = nw->ilu;  // factorised by refresh_jacobian
+      } else if (nw->amg) {
+        nw->prec.kind = LINOP_AMG; nw->prec.amg = nw->amg;   // set up by refresh_jacobian
       } else {
         nw->prec.kind = LINOP_BLOCK_JACOBI;
       }
-      const bool left = o.precond == B200_PRECOND_BLOCK_JACOBI_LEFT || o.precond == B200_PRECOND_MULTIGRID_LEFT || o.precond == B200_PRECOND_ILU0_LEFT;
+      const bool left = o.precond == B200_PRECOND_BLOCK_JACOBI_LEFT || o.precond == B200_PRECOND_MULTIGRID_LEFT || o.precond == B200_PRECOND_ILU0_LEFT ||
+                        o.precond == B200_PRECOND_AMG_LEFT;
       B200_TRY(b200_gmres_set_precond(nw->gm, left ? &nw->prec : nullptr, left ? nullptr : &nw->prec));
     }
     B200_TRY(b200_gmres_solve(nw->gm, &nw->op, nw->fu, nw->xlin, gs));
