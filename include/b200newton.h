@@ -115,9 +115,10 @@ enum { B200_QN_UPDATE_GOOD_BROYDEN = 0, B200_QN_UPDATE_BAD_BROYDEN = 1, B200_QN_
 /* AMG: one Ruge-Stueben algebraic-multigrid V-cycle of the assembled sparse Jacobian (b200_amg_*, default options): hierarchy
    rebuilt at the first fresh Jacobian after create / reinit, values refreshed on the device with every later one; needs
    linsolve = SPARSE_GMRES, any problem with a pattern */
+/* SA_AMG: the same with smoothed aggregation (b200_amg_create_sa, default options): the whole rebuild runs on the device */
 enum { B200_PRECOND_NONE = 0, B200_PRECOND_BLOCK_JACOBI_LEFT = 1, B200_PRECOND_BLOCK_JACOBI_RIGHT = 2,
        B200_PRECOND_MULTIGRID_LEFT = 3, B200_PRECOND_MULTIGRID_RIGHT = 4, B200_PRECOND_ILU0_LEFT = 5, B200_PRECOND_ILU0_RIGHT = 6,
-       B200_PRECOND_AMG_LEFT = 7, B200_PRECOND_AMG_RIGHT = 8 };
+       B200_PRECOND_AMG_LEFT = 7, B200_PRECOND_AMG_RIGHT = 8, B200_PRECOND_SA_AMG_LEFT = 9, B200_PRECOND_SA_AMG_RIGHT = 10 };
 enum { B200_FORCING_NONE = 0, B200_FORCING_EW2 = 1 };
 /* termination modes (public.jl:300-407, termination_conditions.jl:243-372); `du` = f(u).  The three AbsNorm modes keep
    their round-1 values; Norm / Rel / RelNorm / Abs / RelNormSafe / RelNormSafeBest follow */
@@ -389,8 +390,8 @@ int32_t b200_ilu0_linop(b200_ilu0* ilu, b200_linop** op);
  * rules): classical strength (theta), the deterministic first-pass C/F splitting, direct interpolation, Galerkin coarse operators
  * R A P with R = P', an explicit dense inverse of the coarsest level (at most 4096 unknowns).  The pattern (int32 CSR indices,
  * n and every level's nnz < 2^31) is fixed at create.
- *   setup(rebuild = 1): copies the values to the host, chooses the splitting and every pattern there, uploads them, then runs
- *                       the device refresh;  setup(rebuild = 0): the splitting and patterns stay, the device recomputes every
+ *   setup(rebuild = 1): chooses each level's splitting on the host from its values, builds every pattern and value on the device
+ *                       (the coarse values come down for the next splitting), then runs the device refresh;  setup(rebuild = 0): the splitting and patterns stay, the device recomputes every
  *                       value (bit-reproducible; equal bits to a rebuild at the same values).
  *   solve: one V(presweeps, postsweeps) cycle with damped Jacobi from x = 0, replayed as one CUDA graph; a fixed linear operator.
  * info > 0: the 1-based level whose diagonal (or interpolation denominator) is zero or not finite, or whose dense LU met a zero
@@ -404,7 +405,7 @@ typedef struct b200_amg_opts {
   int32_t max_levels;  /* 10 (the finest level counts) */
   int32_t max_coarse;  /* 10: a level of at most this many unknowns is the coarsest */
 } b200_amg_opts;
-enum { B200_AMG_EXPORT_A = 0, B200_AMG_EXPORT_P = 1 };
+enum { B200_AMG_EXPORT_A = 0, B200_AMG_EXPORT_P = 1, B200_AMG_EXPORT_T = 2 /* smoothed aggregation only */ };
 void b200_amg_opts_default(b200_amg_opts* opts);
 /* opts NULL: the defaults.  A row without a structural diagonal fails with B200_ERR_INVALID (the message names the row). */
 int32_t b200_amg_create(b200_ctx* ctx, int64_t n, const int64_t* colptr_host, const int64_t* rowval_host, int32_t index_base,
@@ -414,11 +415,29 @@ int32_t b200_amg_setup(b200_amg* amg, const double* nzval_dev, int32_t rebuild, 
 int32_t b200_amg_solve(b200_amg* amg, const double* b_dev, double* x_dev);  /* x = M^-1 b (x may alias b) */
 /* number of levels; the unknowns and nonzeros of the first `cap` of them */
 int32_t b200_amg_levels(b200_amg* amg, int32_t* nlev_host, int64_t* n_per_level_host, int64_t* nnz_per_level_host, int32_t cap);
-/* the CSR (0-based, int32 indices, columns ascending) of A_level or of P_level (n_level x n_level+1; not on the coarsest level);
-   rowptr holds n_level + 1 entries, col / val rowptr[n_level]; with col and val NULL only rowptr is written */
+/* the CSR (0-based, int32 indices, columns ascending) of A_level, of P_level or (smoothed aggregation) of the tentative
+   prolongator T_level, whose row i holds one entry in the column of i's aggregate or none (n_level x n_level+1; P and T not on
+   the coarsest level); rowptr holds n_level + 1 entries, col / val rowptr[n_level]; with col and val NULL only rowptr is written */
 int32_t b200_amg_export(b200_amg* amg, int32_t level, int32_t what, int32_t* rowptr_host, int32_t* col_host, double* val_host);
 /* an operator applying one V-cycle, for b200_gmres_set_precond; it borrows the handle (destroy the operator first) */
 int32_t b200_amg_linop(b200_amg* amg, b200_linop** op);
+/* Smoothed-aggregation AMG (AlgebraicMultigrid.jl's `smoothed_aggregation`, one candidate; DESIGN.md §4i states the rules):
+ * symmetric strength |a_ij| >= theta sqrt(|a_ii| |a_jj|), aggregates grown from a distance-2 maximal independent set, the
+ * tentative prolongator T (unit columns, b_next = the aggregates' norms of b, b = 1 on the finest level) and
+ * P = T - (smooth_omega / rho) D^-1 A T with rho the Gershgorin bound of D^-1 A.  The handle is a b200_amg: setup, solve, levels,
+ * export and linop work as above, and setup(rebuild = 1) runs on the device with no host pass over the matrix. */
+typedef struct b200_sa_opts {
+  double theta;          /* strength threshold: 0.08 */
+  double omega;          /* Jacobi damping of the cycle: 2/3 */
+  int32_t presweeps;     /* 1 */
+  int32_t postsweeps;    /* 1 */
+  int32_t max_levels;    /* 10 (the finest level counts) */
+  int32_t max_coarse;    /* 10: a level of at most this many unknowns is the coarsest */
+  double smooth_omega;   /* prolongator smoothing weight omega_P: 4/3 */
+} b200_sa_opts;
+void b200_sa_opts_default(b200_sa_opts* opts);
+int32_t b200_amg_create_sa(b200_ctx* ctx, int64_t n, const int64_t* colptr_host, const int64_t* rowval_host, int32_t index_base,
+                           const b200_sa_opts* opts, b200_amg** amg);
 /* the level-0 C/F splitting alone, on the host (no device): cf_out[i] = 1 for a C point, 0 for an F point */
 int32_t b200_amg_split(int64_t n, const int64_t* colptr_host, const int64_t* rowval_host, const double* nzval_host, int32_t index_base,
                        double theta, int32_t* cf_out_host, int64_t* ncoarse_host);

@@ -501,12 +501,17 @@ struct B200ILU0 <: B200Preconditioner end
 the concrete matrix, so it is offered on the whole-solve path only: `B200NewtonKrylov(; linsolve = :sparse_gmres,
 precs = :amg_left | :amg_right)`; `AMGHierarchy` is the stand-alone handle."""
 struct B200AMG <: B200Preconditioner end
+"""`B200SAAMG()`: the same with smoothed aggregation, its whole rebuild on the device: `B200NewtonKrylov(; linsolve = :sparse_gmres,
+precs = :sa_amg_left | :sa_amg_right)`; `AMGHierarchy(ctx, A; method = :smoothed_aggregation)` is the stand-alone handle."""
+struct B200SAAMG <: B200Preconditioner end
 precond_kind(::B200BlockJacobi) = Int32(1)      # B200_PRECOND_BLOCK_JACOBI_LEFT (LEFT / RIGHT of a family name the same operator)
 precond_kind(::B200Multigrid) = Int32(3)        # B200_PRECOND_MULTIGRID_LEFT
 precond_op(::B200ILU0, ::Problem, ::B200Vector) = throw(ArgumentError(
     "B200ILU0 needs the concrete sparse Jacobian: use B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :ilu0_left) (or :ilu0_right)"))
 precond_op(::B200AMG, ::Problem, ::B200Vector) = throw(ArgumentError(
     "B200AMG needs the concrete sparse Jacobian: use B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :amg_left) (or :amg_right)"))
+precond_op(::B200SAAMG, ::Problem, ::B200Vector) = throw(ArgumentError(
+    "B200SAAMG needs the concrete sparse Jacobian: use B200NewtonKrylov(; linsolve = :sparse_gmres, precs = :sa_amg_left) (or :sa_amg_right)"))
 function precond_op(P::B200Preconditioner, prob::Problem, u::B200Vector)
     op = Ref{Ptr{Cvoid}}(C_NULL)
     check(prob.ctx.handle, @ccall libb200.b200_linop_precond(prob.handle::Ptr{Cvoid}, u.ptr::Ptr{Float64}, precond_kind(P)::Int32, op::Ref{Ptr{Cvoid}})::Int32)
@@ -527,20 +532,45 @@ function default_amg_opts()
     @ccall libb200.b200_amg_opts_default(o::Ref{AmgOpts})::Cvoid
     return o[]
 end
+struct SaOpts
+    theta::Float64
+    omega::Float64
+    presweeps::Int32
+    postsweeps::Int32
+    max_levels::Int32
+    max_coarse::Int32
+    smooth_omega::Float64
+end
+function default_sa_opts()
+    o = Ref{SaOpts}()
+    @ccall libb200.b200_sa_opts_default(o::Ref{SaOpts})::Cvoid
+    return o[]
+end
 
-"""`AMGHierarchy(ctx, A::SparseMatrixCSC; opts = default_amg_opts())`: the device Ruge-Stueben hierarchy of A's pattern.
-`setup!(h, nzval; rebuild = true)` returns 0 or the 1-based level of a zero diagonal / pivot; `ldiv!(x, h, b)` applies one
-V-cycle; `amg_levels(h)` the unknowns and nonzeros per level."""
+"""`AMGHierarchy(ctx, A::SparseMatrixCSC; method = :ruge_stuben | :smoothed_aggregation, opts)`: the device algebraic-multigrid
+hierarchy of A's pattern (`opts` an `AmgOpts`, default `default_amg_opts()`, or with smoothed aggregation an `SaOpts`, default
+`default_sa_opts()`).  `setup!(h, nzval; rebuild = true)` returns 0 or the 1-based level of a zero diagonal / pivot; `ldiv!(x, h, b)`
+applies one V-cycle; `amg_levels(h)` the unknowns and nonzeros per level."""
 mutable struct AMGHierarchy
     ctx::Context
     handle::Ptr{Cvoid}
     n::Int
-    function AMGHierarchy(ctx::Context, A::SparseMatrixCSC; opts::AmgOpts = default_amg_opts())
+    function AMGHierarchy(ctx::Context, A::SparseMatrixCSC; method::Symbol = :ruge_stuben,
+                          opts::Union{AmgOpts, SaOpts} = method === :smoothed_aggregation ? default_sa_opts() : default_amg_opts())
         n = size(A, 1)
         h = Ref{Ptr{Cvoid}}(C_NULL)
         colptr, rowval = Vector{Int64}(A.colptr), Vector{Int64}(A.rowval)
-        check(ctx.handle, @ccall libb200.b200_amg_create(ctx.handle::Ctx, n::Int64, colptr::Ptr{Int64}, rowval::Ptr{Int64}, 1::Int32, Ref(opts)::Ref{AmgOpts},
-                                                         h::Ref{Ptr{Cvoid}})::Int32)
+        if method === :smoothed_aggregation
+            opts isa SaOpts || throw(ArgumentError("method = :smoothed_aggregation takes SaOpts"))
+            check(ctx.handle, @ccall libb200.b200_amg_create_sa(ctx.handle::Ctx, n::Int64, colptr::Ptr{Int64}, rowval::Ptr{Int64}, 1::Int32, Ref(opts)::Ref{SaOpts},
+                                                                h::Ref{Ptr{Cvoid}})::Int32)
+        elseif method === :ruge_stuben
+            opts isa AmgOpts || throw(ArgumentError("method = :ruge_stuben takes AmgOpts"))
+            check(ctx.handle, @ccall libb200.b200_amg_create(ctx.handle::Ctx, n::Int64, colptr::Ptr{Int64}, rowval::Ptr{Int64}, 1::Int32, Ref(opts)::Ref{AmgOpts},
+                                                             h::Ref{Ptr{Cvoid}})::Int32)
+        else
+            throw(ArgumentError("method must be :ruge_stuben or :smoothed_aggregation"))
+        end
         H = new(ctx, h[], n)
         finalizer(x -> (@ccall libb200.b200_amg_destroy(x.handle::Ptr{Cvoid})::Int32), H)
         return H
@@ -605,7 +635,7 @@ const _QN_INIT = (identity = 0, true_jacobian = 1, low_rank = 2)
 const _QN_UPDATE = (good_broyden = 0, bad_broyden = 1, klement = 2)
 const _TR_SCHEMES = (simple = 0, nlsolve = 1, nocedal_wright = 2, hei = 3, yuan = 4, fan = 5, bastin = 6)
 const _PRECS = (none = 0, block_jacobi_left = 1, block_jacobi_right = 2, multigrid_left = 3, multigrid_right = 4, ilu0_left = 5, ilu0_right = 6, amg_left = 7,
-    amg_right = 8)
+    amg_right = 8, sa_amg_left = 9, sa_amg_right = 10)
 const _TERMINATION = (abs_norm_safe_best = 0, abs_norm = 1, abs_norm_safe = 2, norm = 3, rel = 4, rel_norm = 5, abs = 6,
     rel_norm_safe = 7, rel_norm_safe_best = 8)
 
@@ -738,7 +768,7 @@ function SciMLBase.__solve(ens::SciMLBase.AbstractEnsembleProblem, alg::B200Newt
     return SciMLBase.EnsembleSolution(sols, time() - t0, converged)
 end
 
-export Context, B200Vector, brusselator, brusselator_function, initial_condition, B200GMRES, B200BlockJacobi, B200Multigrid, B200ILU0, B200AMG, AMGHierarchy, setup!, amg_levels, amg_split,
+export Context, B200Vector, brusselator, brusselator_function, initial_condition, B200GMRES, B200BlockJacobi, B200Multigrid, B200ILU0, B200AMG, B200SAAMG, AMGHierarchy, setup!, amg_levels, amg_split,
     B200NewtonKrylov, EnsembleB200, nccl_unique_id, device_count
 
 end # module

@@ -10,6 +10,6 @@ from .api import (Context, DeviceVector, default_context, device_count, ReturnCo
                   Brusselator2D, Brusselator3D, QuadraticFunction, TridiagQuadFunction, NonlinearFunction, TracerSparsityDetector,
                   NonlinearProblem, remake, KrylovJL_GMRES, LUFactorization, AutoForwardDiff, AutoFiniteDiff, EisenstatWalkerForcing2, BackTracking, BlockJacobi, PseudoTransient, RadiusUpdateSchemes,
                   AbsNormSafeBestTerminationMode, AbsNormSafeTerminationMode, AbsNormTerminationMode, NormTerminationMode, RelTerminationMode, RelNormTerminationMode,
-                  AbsTerminationMode, RelNormSafeTerminationMode, RelNormSafeBestTerminationMode, Multigrid, LevenbergMarquardt, Broyden, LimitedMemoryBroyden, Klement, KLUFactorization, UMFPACKFactorization, SparseBandLU, ILU0, SparseILU0, RugeStubenAMG, SparseAMG, amg_split, NewtonRaphson, TrustRegion,
+                  AbsTerminationMode, RelNormSafeTerminationMode, RelNormSafeBestTerminationMode, Multigrid, LevenbergMarquardt, Broyden, LimitedMemoryBroyden, Klement, KLUFactorization, UMFPACKFactorization, SparseBandLU, ILU0, SparseILU0, RugeStubenAMG, SmoothedAggregationAMG, SparseAMG, amg_split, NewtonRaphson, TrustRegion,
                   SparseJacobian, JacobianOperator, GmresSolver, NonlinearSolveCache, init, step_b, solve_b, reinit_b, EnsembleProblem,
                   EnsembleB200, EnsembleSolution, EnsembleCache, Communicator, shard_range, coloring_column, solve, _DeviceProblem)

@@ -28,7 +28,8 @@ GLOB_NONE, GLOB_TRUST_REGION, GLOB_LINESEARCH = 0, 1, 2
 PRECOND_NONE, PRECOND_BLOCK_JACOBI_LEFT, PRECOND_BLOCK_JACOBI_RIGHT, PRECOND_MULTIGRID_LEFT, PRECOND_MULTIGRID_RIGHT = 0, 1, 2, 3, 4
 PRECOND_ILU0_LEFT, PRECOND_ILU0_RIGHT = 5, 6
 PRECOND_AMG_LEFT, PRECOND_AMG_RIGHT = 7, 8
-AMG_EXPORT_A, AMG_EXPORT_P = 0, 1
+PRECOND_SA_AMG_LEFT, PRECOND_SA_AMG_RIGHT = 9, 10
+AMG_EXPORT_A, AMG_EXPORT_P, AMG_EXPORT_T = 0, 1, 2
 DESCENT_NEWTON, DESCENT_PSEUDO_TRANSIENT, DESCENT_LEVENBERG_MARQUARDT, DESCENT_BROYDEN = 0, 1, 2, 3
 QN_INIT_IDENTITY, QN_INIT_TRUE_JACOBIAN, QN_INIT_LOW_RANK = 0, 1, 2
 QN_UPDATE_GOOD_BROYDEN, QN_UPDATE_BAD_BROYDEN, QN_UPDATE_KLEMENT = 0, 1, 2
@@ -89,6 +90,11 @@ class EnsResult(C.Structure):
 class AmgOpts(C.Structure):
     _fields_ = [("theta", C.c_double), ("omega", C.c_double), ("presweeps", C.c_int32), ("postsweeps", C.c_int32),
                 ("max_levels", C.c_int32), ("max_coarse", C.c_int32)]
+
+
+class SaOpts(C.Structure):
+    _fields_ = [("theta", C.c_double), ("omega", C.c_double), ("presweeps", C.c_int32), ("postsweeps", C.c_int32),
+                ("max_levels", C.c_int32), ("max_coarse", C.c_int32), ("smooth_omega", C.c_double)]
 
 
 RESIDUAL_CB = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p)
@@ -187,6 +193,8 @@ SIGNATURES = {
     "b200_amg_export": (I32, [P, I32, I32, P, P, P]),
     "b200_amg_linop": (I32, [P, PP]),
     "b200_amg_split": (I32, [I64, P, P, P, I32, F64, P, PI64]),
+    "b200_sa_opts_default": (None, [C.POINTER(SaOpts)]),
+    "b200_amg_create_sa": (I32, [P, I64, P, P, I32, C.POINTER(SaOpts), PP]),
     "b200_gmres_solve": (I32, [P, P, P, P, C.POINTER(GmresStats)]),
     "b200_dense_jac_fill": (I32, [P, P, P, I64]),
     "b200_getrf": (I32, [P, I64, P, I64, P, PI32]),

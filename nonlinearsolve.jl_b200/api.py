@@ -443,6 +443,22 @@ class RugeStubenAMG:
         return abi.PRECOND_AMG_LEFT if self.side == "left" else abi.PRECOND_AMG_RIGHT
 
 
+class SmoothedAggregationAMG:
+    """Preconditioner for `KrylovJL_GMRES(precs = ...)` on the concrete sparse Jacobian: one smoothed-aggregation algebraic
+    multigrid V-cycle with damped Jacobi smoothing — the tutorial's `AlgebraicMultigrid.aspreconditioner(smoothed_aggregation(W))`
+    with Jacobi smoothers (docs/src/tutorials/large_systems.md:244-316), default options (theta 0.08, omega 2/3, V(1,1),
+    smooth_omega 4/3).  The aggregates are chosen on the device at the first fresh Jacobian of a solve; later Jacobians refresh
+    every value.  Needs `concrete_jac = True` or a sparse prototype, and serves any problem with a pattern."""
+
+    def __init__(self, side="left"):
+        assert side in ("left", "right")
+        self.side = side
+
+    @property
+    def code(self):
+        return abi.PRECOND_SA_AMG_LEFT if self.side == "left" else abi.PRECOND_SA_AMG_RIGHT
+
+
 class LUFactorization:
     needs_concrete_A = True
 
@@ -525,25 +541,36 @@ class SparseILU0:
 
 
 class SparseAMG:
-    """Direct handle on the device Ruge-Stueben hierarchy of a CSC pattern (colptr, rowval host arrays, 1-based by default).
-    Options: theta, omega, presweeps, postsweeps, max_levels, max_coarse (b200_amg_opts).  `setup(nzval, rebuild=True)` returns
-    0 or the 1-based level of a zero diagonal / pivot (rebuild=False keeps the splitting and recomputes the values), `solve(b)`
-    applies one V-cycle, `levels()` returns the unknowns and nonzeros per level, `level(l)` the CSR arrays of A_l and P_l."""
+    """Direct handle on the device Ruge-Stueben hierarchy of a CSC pattern (colptr, rowval host arrays, 1-based by default), or
+    with `SparseAMG.smoothed_aggregation(...)` the smoothed-aggregation one.
+    Options: theta, omega, presweeps, postsweeps, max_levels, max_coarse (b200_amg_opts; b200_sa_opts adds smooth_omega).
+    `setup(nzval, rebuild=True)` returns 0 or the 1-based level of a zero diagonal / pivot (rebuild=False keeps the splitting or
+    the aggregates and recomputes the values), `solve(b)` applies one V-cycle, `levels()` returns the unknowns and nonzeros per
+    level, `level(l)` the CSR arrays of A_l and P_l (and of the tentative prolongator T_l on smoothed-aggregation handles)."""
 
-    def __init__(self, ctx, n, colptr, rowval, index_base=1, **opts):
+    def __init__(self, ctx, n, colptr, rowval, index_base=1, _method="ruge_stuben", **opts):
         self.ctx, self.n = ctx, n
+        self.method = _method
         colptr = np.ascontiguousarray(colptr, dtype=np.int64)
         rowval = np.ascontiguousarray(rowval, dtype=np.int64)
-        o = abi.AmgOpts()
-        lib().b200_amg_opts_default(C.byref(o))
+        sa = _method == "smoothed_aggregation"
+        o = abi.SaOpts() if sa else abi.AmgOpts()
+        (lib().b200_sa_opts_default if sa else lib().b200_amg_opts_default)(C.byref(o))
         for k, v in opts.items():
-            assert k in dict(abi.AmgOpts._fields_), k
+            assert k in dict(o._fields_), k
             setattr(o, k, v)
         self.opts = o
         self._h = C.c_void_p()
-        check(ctx.handle, lib().b200_amg_create(ctx.handle, n, colptr.ctypes.data_as(C.c_void_p), rowval.ctypes.data_as(C.c_void_p), index_base,
-                                                C.byref(o), C.byref(self._h)))
+        create = lib().b200_amg_create_sa if sa else lib().b200_amg_create
+        check(ctx.handle, create(ctx.handle, n, colptr.ctypes.data_as(C.c_void_p), rowval.ctypes.data_as(C.c_void_p), index_base, C.byref(o),
+                                 C.byref(self._h)))
         self._fin = ctx._adopt(weakref.finalize(self, lib().b200_amg_destroy, self._h))
+
+    @classmethod
+    def smoothed_aggregation(cls, ctx, n, colptr, rowval, index_base=1, **opts):
+        """The smoothed-aggregation hierarchy (b200_amg_create_sa): options theta, omega, presweeps, postsweeps, max_levels,
+        max_coarse, smooth_omega."""
+        return cls(ctx, n, colptr, rowval, index_base, _method="smoothed_aggregation", **opts)
 
     def setup(self, nzval, rebuild=True):
         info = C.c_int32(0)
@@ -572,11 +599,14 @@ class SparseAMG:
         return val, col, rowptr
 
     def level(self, l):
-        """{"A": (data, indices, indptr), "P": ... or None on the coarsest level}: `scipy.sparse.csr_matrix(level["A"])` builds A_l."""
+        """{"A": (data, indices, indptr), "P": ... or None on the coarsest level}: `scipy.sparse.csr_matrix(level["A"])` builds A_l.
+        Smoothed-aggregation handles add "T", the tentative prolongator (None on the coarsest level)."""
         ns, _ = self.levels()
         out = {"A": self._export(l, abi.AMG_EXPORT_A, ns[l]), "P": None}
         if l + 1 < len(ns):
             out["P"] = self._export(l, abi.AMG_EXPORT_P, ns[l])
+        if self.method == "smoothed_aggregation":
+            out["T"] = self._export(l, abi.AMG_EXPORT_T, ns[l]) if l + 1 < len(ns) else None
         return out
 
     def linop(self):

@@ -1507,8 +1507,8 @@ int32_t b200_linop_precond(b200_problem* prob, const double* u, int32_t kind, b2
   if (kind == B200_PRECOND_BLOCK_JACOBI_LEFT || kind == B200_PRECOND_BLOCK_JACOBI_RIGHT) return b200_linop_block_jacobi(prob, u, out);
   B200_REQUIRE(ctx, kind != B200_PRECOND_ILU0_LEFT && kind != B200_PRECOND_ILU0_RIGHT,
                "linop_precond: ILU0 factors the assembled sparse Jacobian, not a problem: use b200_ilu0_create / b200_ilu0_factor / b200_ilu0_linop");
-  B200_REQUIRE(ctx, kind != B200_PRECOND_AMG_LEFT && kind != B200_PRECOND_AMG_RIGHT,
-               "linop_precond: AMG coarsens the assembled sparse Jacobian, not a problem: use b200_amg_create / b200_amg_setup / b200_amg_linop");
+  B200_REQUIRE(ctx, kind != B200_PRECOND_AMG_LEFT && kind != B200_PRECOND_AMG_RIGHT && kind != B200_PRECOND_SA_AMG_LEFT && kind != B200_PRECOND_SA_AMG_RIGHT,
+               "linop_precond: AMG coarsens the assembled sparse Jacobian, not a problem: use b200_amg_create (or b200_amg_create_sa) / b200_amg_setup / b200_amg_linop");
   B200_REQUIRE(ctx, kind == B200_PRECOND_MULTIGRID_LEFT || kind == B200_PRECOND_MULTIGRID_RIGHT, "linop_precond: unknown preconditioner kind");
   b200_mg* mg = nullptr;
   B200_TRY(b200i_mg_create(prob, &mg));

@@ -64,7 +64,7 @@ struct b200_newton {
   b200_sparse_lu* slu;  // LINSOLVE_SPARSE_LU: band factorisation of the assembled Jacobian
   b200_ilu0* ilu;       // PRECOND_ILU0_*: incomplete LU of the assembled Jacobian, refactorised with every fresh J
   int32_t ilu_info;     // its last factorisation: 0, or the 1-based row of a zero / non-finite pivot
-  b200_amg* amg;        // PRECOND_AMG_*: Ruge-Stueben hierarchy of the assembled Jacobian
+  b200_amg* amg;        // PRECOND_AMG_* / PRECOND_SA_AMG_*: Ruge-Stueben or smoothed-aggregation hierarchy of the assembled Jacobian
   int32_t amg_info;     // its last setup: 0, or the 1-based level of a zero diagonal / pivot
   int32_t amg_built;    // a hierarchy exists for this solve: later fresh Jacobians refresh its values (reset by reinit)
   // LevenbergMarquardt: J'J + lambda D'D (factored in place), the running diagonal D'D, velocity / acceleration, previous velocity, J' f
@@ -238,7 +238,8 @@ int32_t b200_newton_destroy(b200_newton* nw) {
 }
 
 static bool ilu0_precond(const b200_newton_opts& o) { return o.precond == B200_PRECOND_ILU0_LEFT || o.precond == B200_PRECOND_ILU0_RIGHT; }
-static bool amg_precond(const b200_newton_opts& o) { return o.precond == B200_PRECOND_AMG_LEFT || o.precond == B200_PRECOND_AMG_RIGHT; }
+static bool sa_precond(const b200_newton_opts& o) { return o.precond == B200_PRECOND_SA_AMG_LEFT || o.precond == B200_PRECOND_SA_AMG_RIGHT; }
+static bool amg_precond(const b200_newton_opts& o) { return o.precond == B200_PRECOND_AMG_LEFT || o.precond == B200_PRECOND_AMG_RIGHT || sa_precond(o); }
 
 // the buffers and sub-solvers b200_newton_create builds for the options; on failure the caller destroys the partial driver
 static int32_t newton_setup(b200_newton* nw) {
@@ -299,7 +300,8 @@ static int32_t newton_setup(b200_newton* nw) {
     // sparse direct route (linsolve = nothing on a sparse prototype): symbolic phase once, like LinearSolve's cache
     if (o.linsolve == B200_LINSOLVE_SPARSE_LU) B200_TRY(b200_sparse_lu_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->slu));
     if (ilu0_precond(o)) B200_TRY(b200_ilu0_create(ctx, n, colptr.data(), rowval.data(), 1, &nw->ilu));
-    if (amg_precond(o)) B200_TRY(b200_amg_create(ctx, n, colptr.data(), rowval.data(), 1, nullptr, &nw->amg));
+    if (sa_precond(o)) B200_TRY(b200_amg_create_sa(ctx, n, colptr.data(), rowval.data(), 1, nullptr, &nw->amg));
+    else if (amg_precond(o)) B200_TRY(b200_amg_create(ctx, n, colptr.data(), rowval.data(), 1, nullptr, &nw->amg));
     nw->op.kind = LINOP_SPARSE_JAC; nw->op.sj = nw->sj; nw->op.nzval = nw->nzval;
   } else {
     return ctx->fail(B200_ERR_INVALID, "unknown linsolve kind", __FILE__, __LINE__);
@@ -325,7 +327,7 @@ int32_t b200_newton_create(b200_problem* prob, const b200_newton_opts* opts, b20
                           (opts->qn_update_rule == B200_QN_UPDATE_KLEMENT && opts->qn_init_jacobian == B200_QN_INIT_IDENTITY))),
                "newton_create: descent must be Newton, PseudoTransient (without a trust region), LevenbergMarquardt (dense concrete Jacobian, its own trust region) or "
                "Broyden (no globalisation, n <= 65535, init_jacobian = true_jacobian needs the dense LU)");
-  B200_REQUIRE(ctx, opts->precond >= B200_PRECOND_NONE && opts->precond <= B200_PRECOND_AMG_RIGHT, "newton_create: unknown preconditioner");
+  B200_REQUIRE(ctx, opts->precond >= B200_PRECOND_NONE && opts->precond <= B200_PRECOND_SA_AMG_RIGHT, "newton_create: unknown preconditioner");
   if (amg_precond(*opts)) {
     // AMG coarsens the assembled sparse Jacobian (any pattern); PseudoTransient's shift changes every step, as for ILU0
     B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_SPARSE_GMRES,
@@ -876,7 +878,7 @@ static int32_t linear_solve(b200_newton* nw, bool fresh, bool* ok, b200_gmres_st
         nw->prec.kind = LINOP_BLOCK_JACOBI;
       }
       const bool left = o.precond == B200_PRECOND_BLOCK_JACOBI_LEFT || o.precond == B200_PRECOND_MULTIGRID_LEFT || o.precond == B200_PRECOND_ILU0_LEFT ||
-                        o.precond == B200_PRECOND_AMG_LEFT;
+                        o.precond == B200_PRECOND_AMG_LEFT || o.precond == B200_PRECOND_SA_AMG_LEFT;
       B200_TRY(b200_gmres_set_precond(nw->gm, left ? &nw->prec : nullptr, left ? nullptr : &nw->prec));
     }
     B200_TRY(b200_gmres_solve(nw->gm, &nw->op, nw->fu, nw->xlin, gs));

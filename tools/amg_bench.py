@@ -1,12 +1,13 @@
-"""Ruge-Stueben AMG as the `precs` of GMRES on the sparse route, measured.   python tools/amg_bench.py [--skip-config4]
+"""Ruge-Stueben and smoothed-aggregation AMG as the `precs` of GMRES on the sparse route, measured.
+    python tools/amg_bench.py [--skip-config4]
 
 Config 4 exactly as bench.py's sparse_tr leg sets it up (3D Brusselator N = 100, coloured sparse Jacobian, TrustRegion, GMRES
-with modified Gram-Schmidt on the assembled matrix), four ways: no preconditioner, ILU0("left"), RugeStubenAMG("left") and
-RugeStubenAMG("right").  Then the AMG alone on config 4's Jacobian at u0: the hierarchy (unknowns and nonzeros per level, operator
-complexity, device bytes it holds), the rebuild (host splitting and patterns, then the device refresh), the refresh, and one
-V-cycle with its bytes/s against the algorithmic bytes defined in `cycle_bytes`.  Last, a user residual with a jac_prototype
-(2D N = 128 periodic diffusion with a cubic reaction, evaluated by torch) with and without AMG.  Prints one JSON line, with the
-card and its power limit."""
+with modified Gram-Schmidt on the assembled matrix), six ways: no preconditioner, ILU0("left"), RugeStubenAMG("left" / "right")
+and SmoothedAggregationAMG("left" / "right").  Then each AMG alone on config 4's Jacobian at u0: the hierarchy (unknowns and
+nonzeros per level, operator complexity, device bytes it holds), the rebuild, the refresh, and one V-cycle with its bytes/s
+against the algorithmic bytes defined in `cycle_bytes`.  Last, a user residual with a jac_prototype (2D N = 128 periodic
+diffusion with a cubic reaction, evaluated by torch) with and without AMG, where the same per-hierarchy numbers are taken on
+the Jacobian at u0.  Prints one JSON line, with the card and its power limit."""
 import json
 import os
 import subprocess
@@ -23,7 +24,9 @@ import nonlinearsolve_jl_b200 as nls  # noqa: E402
 # (as the project's tests do); the right variant keeps the unpreconditioned run's inherited tolerances.
 LEFT = dict(atol=1e-13, rtol=1e-9)
 VARIANTS = (("none", dict()), ("ilu0_left", dict(precs=nls.ILU0("left"), **LEFT)), ("amg_left", dict(precs=nls.RugeStubenAMG("left"), **LEFT)),
-            ("amg_right", dict(precs=nls.RugeStubenAMG("right"))))
+            ("amg_right", dict(precs=nls.RugeStubenAMG("right"))), ("sa_left", dict(precs=nls.SmoothedAggregationAMG("left"), **LEFT)),
+            ("sa_right", dict(precs=nls.SmoothedAggregationAMG("right"))))
+METHODS = (("amg", nls.SparseAMG), ("sa", nls.SparseAMG.smoothed_aggregation))
 
 
 def timed(stream, fn, reps=1, warm=1):
@@ -70,6 +73,30 @@ def cycle_bytes(amg, ns, nzs):
     return total
 
 
+def hierarchy(ctx, stream, make, n, sj, nz):
+    """One AMG alone on the Jacobian values nz: levels, device bytes, rebuild, refresh and one V-cycle."""
+    torch.cuda.synchronize()
+    free0 = torch.cuda.mem_get_info()[0]
+    amg = make(ctx, n, sj.colptr, sj.rowval, 1)
+    t0 = time.perf_counter()
+    rebuild_ms, info = timed(stream, lambda: amg.setup(nz, rebuild=True), warm=0)
+    rebuild_wall_s = time.perf_counter() - t0
+    free1 = torch.cuda.mem_get_info()[0]
+    rebuild2_ms, _ = timed(stream, lambda: amg.setup(nz, rebuild=True), warm=0)
+    refresh_ms, info2 = timed(stream, lambda: amg.setup(nz, rebuild=False), reps=3)
+    b = ctx.to_device(np.random.default_rng(0).standard_normal(n))
+    x = ctx.zeros(n)
+    apply_ms, _ = timed(stream, lambda: amg.solve(b, x), reps=20, warm=2)
+    ns, nzs = amg.levels()
+    nbytes = cycle_bytes(amg, ns, nzs)
+    out = {"nnz": sj.nnz, "levels_n": ns, "levels_nnz": nzs, "operator_complexity": sum(nzs) / nzs[0], "setup_info": [info, info2],
+           "device_bytes_held": free0 - free1, "rebuild_ms": [rebuild_ms, rebuild2_ms], "rebuild_wall_s": rebuild_wall_s, "refresh_ms": refresh_ms,
+           "apply_ms": apply_ms, "apply_bytes": nbytes, "apply_GBps": nbytes / (apply_ms * 1e-3) / 1e9}
+    del amg
+    torch.cuda.empty_cache()
+    return out
+
+
 def config4(ctx, stream):
     N = 100
     f = nls.Brusselator3D(N)
@@ -78,23 +105,9 @@ def config4(ctx, stream):
     out = {"workload": "bruss3d_N100_trustregion_sparse_jacobian_gmres", "unknowns": dp.n}
     sj = nls.SparseJacobian(dp)
     nz = sj.fill(u0)
-    torch.cuda.synchronize()
-    free0 = torch.cuda.mem_get_info()[0]
-    amg = nls.SparseAMG(ctx, dp.n, sj.colptr, sj.rowval, 1)
-    t0 = time.perf_counter()
-    rebuild_ms, info = timed(stream, lambda: amg.setup(nz, rebuild=True), warm=0)
-    rebuild_wall_s = time.perf_counter() - t0
-    free1 = torch.cuda.mem_get_info()[0]
-    refresh_ms, info2 = timed(stream, lambda: amg.setup(nz, rebuild=False), reps=3)
-    b = ctx.to_device(np.random.default_rng(0).standard_normal(dp.n))
-    x = ctx.zeros(dp.n)
-    apply_ms, _ = timed(stream, lambda: amg.solve(b, x), reps=20, warm=2)
-    ns, nzs = amg.levels()
-    nbytes = cycle_bytes(amg, ns, nzs)
-    out["amg"] = {"nnz": sj.nnz, "levels_n": ns, "levels_nnz": nzs, "operator_complexity": sum(nzs) / nzs[0], "setup_info": [info, info2],
-                  "device_bytes_held": free0 - free1, "rebuild_ms": rebuild_ms, "rebuild_wall_s": rebuild_wall_s, "refresh_ms": refresh_ms,
-                  "apply_ms": apply_ms, "apply_bytes": nbytes, "apply_GBps": nbytes / (apply_ms * 1e-3) / 1e9}
-    del amg, sj, nz
+    for key, make in METHODS:
+        out[key] = hierarchy(ctx, stream, make, dp.n, sj, nz)
+    del sj, nz
     torch.cuda.empty_cache()
     fs = nls.NonlinearFunction(f, sparsity=nls.TracerSparsityDetector())
     for name, kw in VARIANTS:
@@ -136,10 +149,16 @@ def user_problem(ctx, stream, N=128):
     fn = nls.NonlinearFunction(F, jvp=JVP, n=n, jac_prototype=(np.array(colptr, dtype=np.int64), np.array(rowval, dtype=np.int64), 1))
     u0 = 0.5 + 0.1 * np.sin(np.arange(n))
     out = {"workload": "user_callback_2d_N%d_jac_prototype_newtonraphson_sparse_gmres" % N, "unknowns": n}
-    for name, kw in (VARIANTS[0], VARIANTS[2], VARIANTS[3]):
+    dp = nls._DeviceProblem(ctx, nls.NonlinearProblem(fn, u0, None, ctx=ctx))
+    sj = nls.SparseJacobian(dp)
+    nz = sj.fill(ctx.to_device(u0))
+    for key, make in METHODS:
+        out[key] = hierarchy(ctx, stream, make, n, sj, nz)
+    del dp, sj, nz
+    for name, kw in (VARIANTS[0],) + VARIANTS[2:]:
         prob = nls.NonlinearProblem(fn, u0, None, ctx=ctx)
         alg = nls.NewtonRaphson(linsolve=nls.KrylovJL_GMRES(**kw))
-        ms, sol = timed(stream, lambda: nls.solve(prob, alg, abstol=1e-9))
+        ms, sol = timed(stream, lambda: nls.solve(prob, alg, abstol=1e-9), reps=3)
         out[name] = summary(ms, sol)
     return out
 
