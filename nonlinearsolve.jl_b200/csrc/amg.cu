@@ -34,6 +34,10 @@ namespace {
 constexpr int AT = 256;
 constexpr int64_t AMG_DENSE_CAP = 4096;  // largest coarsest level that gets an explicit dense inverse
 enum { AMG_RS = 0, AMG_SA = 1 };
+// why coarsening stopped: at max_coarse or max_levels, or stalled: a level with no coarse point / aggregate (no point has a
+// strong connection), or one per unknown (no reduction).  The second is a guard that no input reaches: with any strong
+// connection the Ruge-Stueben pass makes its first pick's dependents F, and a root's graph neighbours are never roots
+enum { AMG_STOP_SIZE = 0, AMG_STOP_NONE = 1, AMG_STOP_ALL = 2 };
 
 // one level of the hierarchy on the device; P, R and the product lists exist on every level but the coarsest
 struct AmgLevel {
@@ -80,6 +84,7 @@ struct b200_amg {
   int64_t* d_ipiv = nullptr;
   int32_t* d_info = nullptr;
   int built = 0, refreshed = 0;
+  int stall = 0;                             // why the last rebuild stopped coarsening (AMG_STOP_*)
   cudaGraphExec_t gexec = nullptr;
   bool graph_unavailable = false;
   int64_t glaunches = 0;
@@ -706,7 +711,7 @@ int32_t rebuild_rs(b200_amg* amg, const double* nzval) {
     std::vector<int32_t> cf, prowptr, pcol, pmap;
     strength(h.n, h.rowptr, h.col, h.val.data(), o.theta, strong);
     const int64_t nc = rs_split(h.n, h.rowptr, h.col, strong, cf);
-    if (nc == 0 || nc == h.n) break;
+    if (nc == 0 || nc == h.n) { amg->stall = nc == 0 ? AMG_STOP_NONE : AMG_STOP_ALL; break; }
     interpolation_pattern(h, strong, cf, prowptr, pcol, pmap);
     AmgLevel& L = amg->lev[l];
     L.pnnz = prowptr[h.n];
@@ -777,7 +782,7 @@ int32_t rebuild_sa(b200_amg* amg, const double* nzval) {
     int32_t na = 0;
     CUDA_TRY(ctx, cudaMemcpyAsync(&na, rid + n, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
-    if (na == 0 || na == n) break;
+    if (na == 0 || na == n) { amg->stall = na == 0 ? AMG_STOP_NONE : AMG_STOP_ALL; break; }
     LAUNCH(ctx, sa_pass1_kernel, blocks(n), AT, 0, n, g, (const uint64_t*)key, (const int32_t*)rid, agg1);
     LAUNCH(ctx, sa_pass2_kernel, blocks(n), AT, 0, n, g, (const int32_t*)agg1, agg2);
     // T: one entry per aggregated row, b / ||b on the aggregate||; the next level's b is the aggregates' norms
@@ -818,13 +823,26 @@ int32_t rebuild_sa(b200_amg* amg, const double* nzval) {
 // either rebuild, then the coarsest level's workspace
 int32_t rebuild(b200_amg* amg, const double* nzval) {
   b200_ctx* ctx = amg->ctx;
+  amg->stall = AMG_STOP_SIZE;
   const int32_t rc = amg->method == AMG_SA ? rebuild_sa(amg, nzval) : rebuild_rs(amg, nzval);
   if (rc != B200_OK) { free_hierarchy(amg); return rc; }
   const int64_t nco = amg->lev.back().n;
   if (nco > AMG_DENSE_CAP) {
-    char msg[256];
-    snprintf(msg, sizeof(msg), "amg_setup: the hierarchy ends at %lld unknowns (%zu levels), above the %lld of the coarsest level's dense inverse: raise max_levels",
-             (long long)nco, amg->lev.size(), (long long)AMG_DENSE_CAP);
+    // the advice names the cause: raising max_levels helps only when max_levels stopped the coarsening
+    char msg[320];
+    const int nlev = (int)amg->lev.size();
+    if (amg->stall != AMG_STOP_SIZE) {
+      const char* why = amg->method == AMG_SA ? (amg->stall == AMG_STOP_NONE ? "no aggregate: no node has a strong connection" : "every node is an aggregate root")
+                                              : (amg->stall == AMG_STOP_NONE ? "no C point: no point has a strong connection" : "every point is a C point");
+      snprintf(msg, sizeof(msg), "amg_setup: coarsening stalls at level %d of %lld unknowns (%s), above the %lld of the coarsest level's dense inverse",
+               nlev, (long long)nco, why, (long long)AMG_DENSE_CAP);
+    } else if (nco <= amg->o.max_coarse) {
+      snprintf(msg, sizeof(msg), "amg_setup: the hierarchy ends at %lld unknowns (%d levels) by max_coarse = %d, above the %lld of the coarsest level's dense inverse: lower max_coarse",
+               (long long)nco, nlev, (int)amg->o.max_coarse, (long long)AMG_DENSE_CAP);
+    } else {
+      snprintf(msg, sizeof(msg), "amg_setup: the hierarchy ends at %lld unknowns (%d levels), above the %lld of the coarsest level's dense inverse: raise max_levels",
+               (long long)nco, nlev, (long long)AMG_DENSE_CAP);
+    }
     free_hierarchy(amg);
     return ctx->fail(B200_ERR_UNSUPPORTED, msg, __FILE__, __LINE__);
   }
