@@ -457,7 +457,11 @@ int32_t b200_newton_trace(b200_newton* nw, b200_trace_rec* recs_host, int32_t ca
 int32_t b200_newton_solve_host(b200_newton* nw, const double* u0_host, double* u_host, double* resid_host,
                                b200_newton_result* result_host);
 
-/* ---------------------------------------------------------------- ensemble (a11): K independent 2D Brusselators */
+/* ---------------------------------------------------------------- ensemble (a11): K independent 2D Brusselators
+ * Trajectories are matrix-free NewtonRaphson solves with GMRES.  The preconditioner may be none, block-Jacobi or multigrid
+ * (either side); ILU0 and AMG need the assembled sparse Jacobian and are refused with B200_ERR_INVALID.  For N <= 32 one kernel
+ * solves the whole batch, one CTA per trajectory, with the multigrid V-cycle in shared memory; block-Jacobi, N > 32 and the
+ * option sets that kernel does not cover run the single-system driver, one trajectory after another. */
 typedef struct b200_ens_result {
   int32_t nprob;
   int32_t nsuccess;
@@ -473,6 +477,13 @@ int32_t b200_ens_destroy(b200_ensemble* ens);
 int32_t b200_ens_solve(b200_ensemble* ens, const double* u0_dev, const double* A_dev, const double* B_dev, double* u_out_dev,
                        double* resid_inf_dev, int32_t* retcodes_dev, int32_t* nsteps_dev, int32_t* njvp_dev,
                        b200_ens_result* result_host);
+/* y_m = M_m^-1 x_m for every trajectory m of a batched multigrid ensemble: M_m is the V-cycle at iterate u_m with parameter
+   A_m, applied by the solve kernel's own device routine (u, x, y: nprob x n like u0; A: nprob).  B200_ERR_INVALID for any
+   other ensemble. */
+int32_t b200_ens_precond_apply(b200_ensemble* ens, const double* u_dev, const double* A_dev, const double* x_dev, double* y_dev);
+/* resident CTAs per SM of the batched solve kernel for this ensemble's options (the occupancy query that sizes its grid);
+   0 when its trajectories take the single-system driver */
+int32_t b200_ens_ctas_per_sm(b200_ensemble* ens, int32_t* ctas_per_sm);
 
 /* ---------------------------------------------------------------- collective step of the ensemble path (SURVEY.md §8b, §8e)
  * The ensemble shards by contiguous trajectory blocks, rank r owning [r K/R, (r+1) K/R): no collective on the data path.

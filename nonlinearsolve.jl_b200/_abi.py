@@ -223,6 +223,8 @@ SIGNATURES = {
     "b200_ens_create": (I32, [P, I32, I32, F64, C.POINTER(NewtonOpts), PP]),
     "b200_ens_destroy": (I32, [P]),
     "b200_ens_solve": (I32, [P, P, P, P, P, P, P, P, P, C.POINTER(EnsResult)]),
+    "b200_ens_precond_apply": (I32, [P, P, P, P, P]),
+    "b200_ens_ctas_per_sm": (I32, [P, PI32]),
     "b200_nccl_version": (I32, [PI32]),
     "b200_nccl_unique_id": (I32, [P]),
     "b200_nccl_init": (I32, [P, I32, I32, P, PP]),

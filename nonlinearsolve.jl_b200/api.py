@@ -1292,8 +1292,10 @@ def shard_range(K, rank, world_size):
 
 
 class EnsembleCache:
-    """Persistent per-GPU batch workspace for K_local 2D-Brusselator trajectories.  The options are those of a single solve;
-    option sets the batched kernel does not implement (see csrc/ens_batched.cu) run each trajectory through the general driver."""
+    """Persistent per-GPU batch workspace for K_local 2D-Brusselator trajectories.  The options are those of a single solve,
+    preconditioner included (`Multigrid` on either side is batched, `BlockJacobi` runs trajectory by trajectory; ILU0 and the
+    AMGs need an assembled Jacobian and are refused); option sets the batched kernel does not implement (see
+    csrc/ens_batched.cu) run each trajectory through the general driver."""
 
     def __init__(self, ctx, N, nprob_local, alpha, alg, abstol=None, reltol=None, maxiters=1000, termination_condition=None, maxtime=None):
         self.ctx, self.N, self.K, self.n = ctx, N, nprob_local, 2 * N * N
@@ -1313,6 +1315,19 @@ class EnsembleCache:
         check(self.ctx.handle, lib().b200_ens_solve(self._h, u0_dev.ptr, A_dev.ptr, B_dev.ptr, self.u_out.ptr, self.resid.ptr, self.rc.ptr,
                                                     self.ns.ptr, self.nj.ptr, C.byref(res)))
         return res
+
+    def precond_apply(self, u_dev, A_dev, x_dev, y_dev=None):
+        """y_m = M_m^-1 x_m for every trajectory of a batched multigrid ensemble, M_m the V-cycle at iterate u_m with parameter
+        A_m, by the solve kernel's own routine (u, x, y: K x n device vectors, A: K).  Returns y."""
+        y_dev = self.ctx.empty(self.K * self.n) if y_dev is None else y_dev
+        check(self.ctx.handle, lib().b200_ens_precond_apply(self._h, u_dev.ptr, A_dev.ptr, x_dev.ptr, y_dev.ptr))
+        return y_dev
+
+    def ctas_per_sm(self):
+        """Resident CTAs per SM of the batched solve kernel for these options (0 when trajectories take the general driver)."""
+        v = C.c_int32()
+        check(self.ctx.handle, lib().b200_ens_ctas_per_sm(self._h, C.byref(v)))
+        return v.value
 
 
 class Communicator:

@@ -7,10 +7,12 @@
 // trajectory in the reference (test/PolyAlgorithms/core_tests__item6.jl:3-20).
 //
 // Option sets batched here (b200i_ens_batched_supported): exact JVP; unrestarted GMRES with MGS or CGS2 (MGS applied twice),
-// any itmax / atol / rtol, optional EW forcing; termination AbsNorm, AbsNormSafe or AbsNormSafeBest on the inf-norm with the
-// default step-stall window (32); no maxtime; N <= 32.  Every other option set (the Norm / Rel / Abs modes, the L2 norm,
-// another stall window, one-pass CGS, a wall-clock limit, FD-JVP, warm start, restart, N > 32) runs each trajectory
-// through the general driver of newton.cu instead (b200_ens_solve).  tests/test_gpu_ensemble.py checks both routes.
+// any itmax / atol / rtol, optional EW forcing; no preconditioner, or the multigrid V-cycle of mg.cu on either side
+// (Multigrid("left") / Multigrid("right")); termination AbsNorm, AbsNormSafe or AbsNormSafeBest on the inf-norm with the
+// default step-stall window (32); no maxtime; N <= 32.  Every other option set (block-Jacobi, the Norm / Rel / Abs modes, the
+// L2 norm, another stall window, one-pass CGS, a wall-clock limit, FD-JVP, warm start, restart, N > 32) runs each trajectory
+// through the general driver of newton.cu instead (b200_ens_solve).  tests/test_gpu_ensemble.py and
+// tests/test_gpu_ensemble_precond.py check both routes.
 //
 // Design: a 2D N=32 trajectory has n = 2048 unknowns = 16 KB per vector, so a CTA owns a whole trajectory:
 //   * iterate u and the current Krylov direction v_k live in shared memory (stencil neighbourhoods are read from there),
@@ -23,7 +25,17 @@
 //     no host round trip, no grid-wide synchronisation, no lock step between trajectories (converged CTAs fetch the
 //     next trajectory from an atomic work queue).
 // Algorithmic HBM bytes per Arnoldi step j: passes * j * Bv (basis) + Bv (store v_{j+1}) + j * 8 (R column), Bv = 8 n.
+//
+// Multigrid (ens_newton_kernel<ENS_PC_MG_LEFT / ENS_PC_MG_RIGHT>): the whole hierarchy of mg.cu (N -> N / p for the smallest
+// prime factor p, down to one cell) lives in shared memory beside the iterate: per level the restricted state and two iterate
+// buffers, and on the coarse levels the right-hand side (the fine level's is v_k).  Each Newton step restricts the iterate
+// level by level (b200i_mg_setup); each application is one V-cycle with one cell per thread per level and one barrier per
+// sweep, built from the per-cell functions of mg_cell.cuh, so it rounds exactly like the single-system preconditioner.  GMRES
+// follows the driver (Krylov.jl gmres!(; M, N, ldiv = false)): right w = J M^-1 v_k and x = M^-1 V_k y; left r0 = M^-1 f,
+// w = M^-1 J v_k, the tolerance atol + rtol ||M^-1 f|| while Eisenstat-Walker keeps ||f||_2.  V-cycles are not matvecs:
+// njvp counts Arnoldi steps, as the driver's does.
 #include "common.cuh"
+#include "mg_cell.cuh"
 #include <algorithm>
 #include <cstdlib>
 #include <math.h>
@@ -32,6 +44,16 @@ namespace {
 constexpr int ENS_LS_BASIS_FULL = 100;  // internal GMRES stop code: the per-CTA basis slab is full (never leaves this file)
 constexpr int ET = 256;   // threads per CTA
 constexpr int NPT = 8;    // max rows per thread  -> n <= 2048 (N <= 32)
+constexpr int ENS_PC_NONE = 0, ENS_PC_MG_LEFT = 1, ENS_PC_MG_RIGHT = 2;  // preconditioner of a kernel instantiation
+constexpr int ENS_MG_MAXLEV = 8;   // 2D N <= 32: at most 32 -> 16 -> 8 -> 4 -> 2 -> 1
+constexpr double ENS_MG_OMEGA = 0.8;
+
+// One multigrid level: points per dimension, ratio to the next level (0 on the last), Laplacian coefficient, and where its
+// buffers sit in dynamic shared memory (offsets in doubles; level 0's state is the iterate, its right-hand side the caller's)
+struct EnsMgLevel {
+  double a;
+  int N, ratio, st, x, x2, b;
+};
 
 struct EnsParams {
   int N, n, nprob, maxiters, itmax, kcap, passes, term_mode, forcing, ew_safeguard;
@@ -40,6 +62,9 @@ struct EnsParams {
   double ew_eta0, ew_eta_max, ew_gamma, ew_alpha, ew_safeguard_threshold;
   int64_t slab;  // doubles per CTA workspace slab
   int npad;
+  int mg_nlev, mg_tab;             // multigrid: number of levels, offset (doubles) of the level table in shared memory
+  int mg_doubles;                  // multigrid: shared-memory doubles of the table and every level's buffers
+  EnsMgLevel mg[ENS_MG_MAXLEV];
 };
 
 struct CtaState {  // shared-memory scalars, written by thread 0, read after a barrier
@@ -141,6 +166,81 @@ __device__ __forceinline__ void ens_jvp(const EnsParams& P, double A, const doub
   }
 }
 
+// ---- the multigrid V-cycle of mg.cu on one CTA, every level in shared memory
+// One sweep of the level operator (mg_op_cell MODE), one cell per thread, then one barrier (the sweeps ping-pong between
+// two buffers, so no barrier is needed between the reads and the writes of a sweep).
+template <int MODE>
+__device__ __forceinline__ void ens_mg_sweep(const EnsMgLevel& L, double A, const double* st, const double* x, const double* b, double* out,
+                                             double omega) {
+  const int N = L.N, NC = N * N;
+  const double a = L.a;
+  for (int c = threadIdx.x; c < NC; c += ET) mg_op_cell<MODE, int>(c, N, 2, NC, a, A, st, x, b, out, omega);
+  __syncthreads();
+}
+
+// b200i_mg_setup: restrict the iterate (level 0's state) level by level
+__device__ __forceinline__ void ens_mg_setup(double* sm, const EnsMgLevel* lev, int nlev) {
+  for (int l = 0; l + 1 < nlev; ++l) {
+    const int Nf = lev[l].N, Nc = lev[l + 1].N, ratio = lev[l].ratio;
+    const double* fine = sm + lev[l].st;
+    double* coarse = sm + lev[l + 1].st;
+    for (int c = threadIdx.x; c < Nc * Nc; c += ET) mg_restrict_cell<int>(c, Nf, Nc, 2, ratio, fine, coarse);
+    __syncthreads();
+  }
+}
+
+// M^-1 b0 by one V-cycle (mg_vcycle of mg.cu, unrolled from the recursion): nu pre-sweeps (the first from the zero guess),
+// residual, restriction, the coarse cycle, prolongation, nu post-sweeps; the one-cell level is the exact 2x2 solve.  b0 is
+// the fine right-hand side in shared memory and is only read.  Returns the fine-level buffer that holds the result; it stays
+// valid until the next call.
+__device__ __forceinline__ const double* ens_vcycle(double* sm, const EnsMgLevel* lev, int nlev, double A, const double* b0) {
+  const double* b = b0;
+  for (int l = 0; l + 1 < nlev; ++l) {
+    const EnsMgLevel& L = lev[l];
+    const double* st = sm + L.st;
+    double* cur = sm + L.x;
+    double* nxt = sm + L.x2;
+    const int nu = L.ratio == 2 ? 2 : 2 * L.ratio;
+    ens_mg_sweep<3>(L, A, st, nullptr, b, cur, ENS_MG_OMEGA);
+    for (int s = 1; s < nu; ++s) { ens_mg_sweep<2>(L, A, st, cur, b, nxt, ENS_MG_OMEGA); double* t = cur; cur = nxt; nxt = t; }
+    ens_mg_sweep<1>(L, A, st, cur, b, nxt, 0.0);  // residual into the free buffer
+    const int Nc = lev[l + 1].N;
+    double* bc = sm + lev[l + 1].b;
+    for (int c = threadIdx.x; c < Nc * Nc; c += ET) mg_restrict_cell<int>(c, L.N, Nc, 2, L.ratio, nxt, bc);
+    __syncthreads();
+    b = bc;
+  }
+  const EnsMgLevel& Ll = lev[nlev - 1];
+  double* cur = sm + Ll.x;
+  double* nxt = sm + Ll.x2;
+  ens_mg_sweep<3>(Ll, A, sm + Ll.st, nullptr, b, cur, Ll.N == 1 ? 1.0 : ENS_MG_OMEGA);
+  if (Ll.N > 1)  // a grid that cannot be coarsened: smoothing only
+    for (int s = 0; s < 7; ++s) { ens_mg_sweep<2>(Ll, A, sm + Ll.st, cur, b, nxt, ENS_MG_OMEGA); double* t = cur; cur = nxt; nxt = t; }
+  const double* xc = cur;
+  for (int l = nlev - 2; l >= 0; --l) {
+    const EnsMgLevel& L = lev[l];
+    const double* st = sm + L.st;
+    const double* bl = l == 0 ? b0 : sm + L.b;
+    const int nu = L.ratio == 2 ? 2 : 2 * L.ratio;
+    cur = sm + (((nu - 1) & 1) ? L.x2 : L.x);  // where the pre-smoothing left the iterate
+    nxt = sm + (((nu - 1) & 1) ? L.x : L.x2);
+    const int Nc = lev[l + 1].N;
+    for (int c = threadIdx.x; c < L.N * L.N; c += ET) mg_prolong_add_cell<int>(c, L.N, Nc, 2, L.ratio, xc, cur);
+    __syncthreads();
+    for (int s = 0; s < nu; ++s) { ens_mg_sweep<2>(L, A, st, cur, bl, nxt, ENS_MG_OMEGA); double* t = cur; cur = nxt; nxt = t; }
+    xc = cur;
+  }
+  return xc;
+}
+
+// the level table from the kernel parameters into shared memory (constant indices only); visible after the next barrier
+__device__ __forceinline__ void ens_mg_load_table(const EnsParams& P, EnsMgLevel* mgl) {
+#pragma unroll
+  for (int l = 0; l < ENS_MG_MAXLEV; ++l)
+    if ((int)threadIdx.x == l) mgl[l] = P.mg[l];
+}
+
+template <int PC>
 __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const double* __restrict__ u0, const double* __restrict__ Aarr,
                                                             const double* __restrict__ Barr, const double* __restrict__ forcing,
                                                             double* __restrict__ u_out, double* __restrict__ resid_inf,
@@ -156,6 +256,8 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
   double* obj_trace = zs + P.kcap + 2;  // [100]
   double* step_trace = obj_trace + 100; // [32]
   double(*red)[ET / 32] = reinterpret_cast<double(*)[ET / 32]>(step_trace + 32);  // [2][8]
+  EnsMgLevel* mgl = reinterpret_cast<EnsMgLevel*>(sm + P.mg_tab);                // multigrid: level table, then the levels
+  if constexpr (PC != ENS_PC_NONE) ens_mg_load_table(P, mgl);
   __shared__ CtaState st;
   __shared__ int cur_problem;
   int phase = 0;
@@ -192,9 +294,9 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
       double fsq = 0.0;
 #pragma unroll
       for (int q = 0; q < NPT; ++q) fsq = fma(f[q], f[q], fsq);
-      const double beta = sqrt(blk_sum_all(fsq, red, phase));
+      const double fnorm = sqrt(blk_sum_all(fsq, red, phase));
       if (P.forcing) {  // eisenstat_walker.jl:42-87 (internalnorm = L2)
-        if (nsteps == 0) { eta = P.ew_eta0; rnorm_nl = rnorm_nl_prev = beta; }
+        if (nsteps == 0) { eta = P.ew_eta0; rnorm_nl = rnorm_nl_prev = fnorm; }
         else {
           const double eta_prev = eta;
           eta = P.ew_gamma * pow(rnorm_nl / rnorm_nl_prev, P.ew_alpha);
@@ -203,7 +305,19 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
         }
         gm_rtol = eta;
         rnorm_nl_prev = rnorm_nl;  // post_step_forcing!: fu is still the residual at the pre-update iterate
-        rnorm_nl = beta;
+        rnorm_nl = fnorm;
+      }
+      double beta = fnorm;  // GMRES's ||r0||
+      if constexpr (PC != ENS_PC_NONE) ens_mg_setup(sm, mgl, P.mg_nlev);  // the hierarchy follows the linearisation point
+      if constexpr (PC == ENS_PC_MG_LEFT) {  // r0 = M^-1 f: the iteration and its stopping test live in the preconditioned space
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) vk[r] = f[q]; }
+        __syncthreads();
+        const double* g = ens_vcycle(sm, mgl, P.mg_nlev, A, vk);
+        double gsq = 0.0;
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; f[q] = (r < n) ? g[r] : 0.0; gsq = fma(f[q], f[q], gsq); }
+        beta = sqrt(blk_sum_all(gsq, red, phase));
       }
       const double tol = P.gm_atol + gm_rtol * beta;
       int gstatus = 0, k = 0;
@@ -222,7 +336,20 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
       while (gstatus == 0) {
         ++k;
         double w[NPT];
-        ens_jvp(P, A, us, vk, w);
+        if constexpr (PC == ENS_PC_MG_RIGHT) {  // w = J M^-1 v_k
+          ens_jvp(P, A, us, ens_vcycle(sm, mgl, P.mg_nlev, A, vk), w);
+        } else {
+          ens_jvp(P, A, us, vk, w);
+        }
+        if constexpr (PC == ENS_PC_MG_LEFT) {  // w = M^-1 J v_k: J v_k goes through vk, which is free until v_{k+1} is stored
+          __syncthreads();
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) vk[r] = w[q]; }
+          __syncthreads();
+          const double* z = ens_vcycle(sm, mgl, P.mg_nlev, A, vk);
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; w[q] = (r < n) ? z[r] : 0.0; }
+        }
         ++njvp;
         // ---- (iterated) modified Gram-Schmidt, one basis read per pass
         for (int pass = 0; pass < P.passes; ++pass) {
@@ -314,6 +441,16 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
 #pragma unroll
         for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) x[q] = fma(yi, vi[r], x[q]); }
       }
+      if constexpr (PC == ENS_PC_MG_RIGHT) {  // x = M^-1 (V_k y)
+        if (k > 0) {
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) vk[r] = x[q]; }
+          __syncthreads();
+          const double* z = ens_vcycle(sm, mgl, P.mg_nlev, A, vk);
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) x[q] = z[r]; }
+        }
+      }
       // ================= u += du, du = -x ; fu = f(u) ; termination (solve.jl:436-452) =================
       double dsq = 0.0;
       __syncthreads();
@@ -388,30 +525,50 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
   }
 }
 
+// y_m = M_m^-1 x_m for trajectory m = blockIdx.x: the solve kernel's setup and V-cycle on the same shared-memory layout
+__global__ void __launch_bounds__(ET, 2) ens_precond_apply_kernel(EnsParams P, const double* __restrict__ u, const double* __restrict__ Aarr,
+                                                                   const double* __restrict__ x, double* __restrict__ y) {
+  extern __shared__ double sm[];
+  double* us = sm;
+  double* vk = us + P.npad;
+  EnsMgLevel* mgl = reinterpret_cast<EnsMgLevel*>(sm + P.mg_tab);
+  ens_mg_load_table(P, mgl);
+  const int m = blockIdx.x, n = P.n;
+  const double A = Aarr[m];
+  for (int r = threadIdx.x; r < n; r += ET) { us[r] = u[(int64_t)m * n + r]; vk[r] = x[(int64_t)m * n + r]; }
+  __syncthreads();
+  ens_mg_setup(sm, mgl, P.mg_nlev);
+  const double* z = ens_vcycle(sm, mgl, P.mg_nlev, A, vk);
+  for (int r = threadIdx.x; r < n; r += ET) y[(int64_t)m * n + r] = z[r];
+}
+
 size_t ens_smem_bytes(const EnsParams& P) {
-  return sizeof(double) * ((size_t)2 * P.npad + 4 * (size_t)(P.kcap + 2) + 100 + 32 + 2 * (ET / 32));
-}
-}  // namespace
-
-// The option sets the kernel implements exactly; everything else goes to the general driver (b200_ens_solve's sequential route).
-// Termination: the three AbsNorm modes on the inf-norm, with the Safe modes' step-stall window at its default of 32 (the
-// window is fixed in the kernel; a non-Safe mode has none, so its setting does not matter).  No wall-clock limit.
-int32_t b200i_ens_batched_supported(int32_t N, const b200_newton_opts* o) {
-  if (2 * N * N > ET * NPT) return 0;
-  if (o->jvp_mode != B200_JVP_EXACT || o->gmres.warm_start || o->gmres.restart > 0) return 0;
-  if (o->gmres.orth != B200_ORTH_MGS && o->gmres.orth != B200_ORTH_CGS2) return 0;
-  const int t = o->termination;
-  if (t != B200_TERM_ABS_NORM && t != B200_TERM_ABS_NORM_SAFE && t != B200_TERM_ABS_NORM_SAFE_BEST) return 0;
-  if (o->term_norm != B200_NORM_INF) return 0;
-  if (t != B200_TERM_ABS_NORM && o->term_max_stalled_steps != 0 && o->term_max_stalled_steps != 32) return 0;
-  if (o->maxtime > 0.0) return 0;
-  return 1;
+  return sizeof(double) * ((size_t)2 * P.npad + 4 * (size_t)(P.kcap + 2) + 100 + 32 + 2 * (ET / 32) + (size_t)P.mg_doubles);
 }
 
-int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double alpha, const b200_newton_opts* o, const double* u0,
-                                const double* A, const double* B, double* u_out, double* resid_inf, int32_t* retcodes, int32_t* nsteps,
-                                int32_t* njvp, void** workspace, size_t* workspace_bytes, int32_t* n_deferred) {
-  EnsParams P;
+int ens_pc(const b200_newton_opts* o) {
+  return o->precond == B200_PRECOND_MULTIGRID_LEFT ? ENS_PC_MG_LEFT : o->precond == B200_PRECOND_MULTIGRID_RIGHT ? ENS_PC_MG_RIGHT : ENS_PC_NONE;
+}
+
+using EnsKernel = void (*)(EnsParams, const double*, const double*, const double*, const double*, double*, double*, int32_t*, int32_t*,
+                           int32_t*, double*, int*);
+EnsKernel ens_kernel(int pc) {
+  return pc == ENS_PC_MG_LEFT ? ens_newton_kernel<ENS_PC_MG_LEFT> : pc == ENS_PC_MG_RIGHT ? ens_newton_kernel<ENS_PC_MG_RIGHT>
+                                                                                          : ens_newton_kernel<ENS_PC_NONE>;
+}
+
+int smallest_factor(int n) {
+  for (int p = 2; p * p <= n; ++p)
+    if (n % p == 0) return p;
+  return n;
+}
+
+// The kernel parameters of an option set.  With multigrid, the hierarchy of b200i_mg_create for a 2D N <= 32 grid (it always
+// reaches one cell: no prime N > 7 has more than 4096 cells here) and its shared-memory plan after the unpreconditioned
+// layout: the level table, level 0's two iterate buffers (its state is u, its right-hand side v_k), then per coarse level
+// state, x, x2 and b, 2 N_l^2 doubles each.
+void ens_params(int32_t N, int32_t nprob, double alpha, const b200_newton_opts* o, EnsParams* out) {
+  EnsParams& P = *out;
   memset(&P, 0, sizeof(P));
   P.N = N; P.n = 2 * N * N; P.nprob = nprob;
   P.walk_di = ET % N; P.walk_dj = ET / N;
@@ -435,10 +592,66 @@ int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double 
   const double dx = 1.0 / (double)(N - 1);
   P.a = alpha / (dx * dx);
   P.slab = (int64_t)(P.kcap + 1) * P.npad + (int64_t)P.kcap * (P.kcap + 1) / 2 + 16;
+  if (ens_pc(o) != ENS_PC_NONE) {
+    P.mg_tab = 2 * P.npad + 4 * (P.kcap + 2) + 100 + 32 + 2 * (ET / 32);
+    int off = P.mg_tab + (int)(sizeof(EnsMgLevel) / sizeof(double)) * ENS_MG_MAXLEV;
+    int Nl = N;
+    double a = P.a;
+    for (int l = 0;; ++l) {
+      EnsMgLevel& L = P.mg[l];
+      L.N = Nl; L.a = a;
+      L.ratio = Nl > 1 ? smallest_factor(Nl) : 0;
+      const int len = 2 * Nl * Nl;
+      if (l == 0) { L.st = 0; L.b = -1; L.x = off; L.x2 = off + P.npad; off += 2 * P.npad; }
+      else { L.st = off; L.x = off + len; L.x2 = off + 2 * len; L.b = off + 3 * len; off += 4 * len; }
+      P.mg_nlev = l + 1;
+      if (L.ratio == 0) break;
+      Nl /= L.ratio;
+      a /= (double)L.ratio * L.ratio;  // b200i_mg_create's a_l, divided in the same order
+    }
+    P.mg_doubles = off - P.mg_tab;
+  }
+}
+}  // namespace
+
+// The option sets the kernel implements exactly; everything else goes to the general driver (b200_ens_solve's sequential route).
+// Termination: the three AbsNorm modes on the inf-norm, with the Safe modes' step-stall window at its default of 32 (the
+// window is fixed in the kernel; a non-Safe mode has none, so its setting does not matter).  No wall-clock limit.
+int32_t b200i_ens_batched_supported(int32_t N, const b200_newton_opts* o) {
+  if (2 * N * N > ET * NPT) return 0;
+  if (o->precond != B200_PRECOND_NONE && ens_pc(o) == ENS_PC_NONE) return 0;  // block-Jacobi: the driver, trajectory by trajectory
+  if (o->jvp_mode != B200_JVP_EXACT || o->gmres.warm_start || o->gmres.restart > 0) return 0;
+  if (o->gmres.orth != B200_ORTH_MGS && o->gmres.orth != B200_ORTH_CGS2) return 0;
+  const int t = o->termination;
+  if (t != B200_TERM_ABS_NORM && t != B200_TERM_ABS_NORM_SAFE && t != B200_TERM_ABS_NORM_SAFE_BEST) return 0;
+  if (o->term_norm != B200_NORM_INF) return 0;
+  if (t != B200_TERM_ABS_NORM && o->term_max_stalled_steps != 0 && o->term_max_stalled_steps != 32) return 0;
+  if (o->maxtime > 0.0) return 0;
+  return 1;
+}
+
+// Resident CTAs per SM of the solve kernel for this option set (the occupancy query that sizes its persistent grid)
+int32_t b200i_ens_batched_ctas_per_sm(b200_ctx* ctx, int32_t N, const b200_newton_opts* o, int32_t* per_sm) {
+  EnsParams P;
+  ens_params(N, 1, 1.0, o, &P);
   const size_t smem = ens_smem_bytes(P);
-  CUDA_TRY(ctx, cudaFuncSetAttribute(ens_newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const EnsKernel kernel = ens_kernel(ens_pc(o));
+  CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int v = 0;
+  CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kernel, ET, smem));
+  *per_sm = v;
+  return B200_OK;
+}
+
+int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double alpha, const b200_newton_opts* o, const double* u0,
+                                const double* A, const double* B, double* u_out, double* resid_inf, int32_t* retcodes, int32_t* nsteps,
+                                int32_t* njvp, void** workspace, size_t* workspace_bytes, int32_t* n_deferred) {
+  EnsParams P;
+  ens_params(N, nprob, alpha, o, &P);
+  const size_t smem = ens_smem_bytes(P);
+  const EnsKernel kernel = ens_kernel(ens_pc(o));
   int per_sm = 0;
-  CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ens_newton_kernel, ET, smem));
+  B200_TRY(b200i_ens_batched_ctas_per_sm(ctx, N, o, &per_sm));
   if (per_sm < 1) return ctx->fail(B200_ERR_UNSUPPORTED, "ensemble kernel does not fit on an SM", __FILE__, __LINE__);
   const int grid = std::min(nprob, per_sm * ctx->sm_count);
   // workspace: per-CTA slabs + the forcing plane + the work-queue counter
@@ -463,7 +676,7 @@ int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double 
   CUDA_TRY(ctx, cudaMemcpyAsync(d_forcing, forcing.data(), sizeof(double) * forcing.size(), cudaMemcpyHostToDevice, ctx->stream));
   CUDA_TRY(ctx, cudaMemsetAsync(d_counter, 0, 2 * sizeof(int), ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // `forcing` is a host temporary
-  PLAUNCH(ctx, B200_KID_RESIDENT, 0.0, ens_newton_kernel, grid, ET, smem, P, u0, A, B, (const double*)d_forcing, u_out, resid_inf, retcodes, nsteps,
+  PLAUNCH(ctx, B200_KID_RESIDENT, 0.0, kernel, grid, ET, smem, P, u0, A, B, (const double*)d_forcing, u_out, resid_inf, retcodes, nsteps,
           njvp, ws, d_counter);
   CHECK_LAUNCH(ctx);
   // trajectories whose Krylov basis outgrew the per-CTA slab (kcap < min(itmax, n)) come back marked B200I_ENS_RC_DEFERRED
@@ -471,5 +684,19 @@ int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double 
   CUDA_TRY(ctx, cudaMemcpyAsync(&hits, d_counter + 1, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   *n_deferred = hits;
+  return B200_OK;
+}
+
+// y_m = M_m^-1 x_m for every trajectory (u, A, x, y: nprob trajectories, problem-major), one CTA per trajectory: the V-cycle
+// of the multigrid solve kernel, for a caller to check it against the single-system preconditioner
+int32_t b200i_ens_batched_precond_apply(b200_ctx* ctx, int32_t N, int32_t nprob, double alpha, const b200_newton_opts* o, const double* u,
+                                        const double* A, const double* x, double* y) {
+  EnsParams P;
+  ens_params(N, nprob, alpha, o, &P);
+  B200_REQUIRE(ctx, P.mg_nlev > 0, "ens_precond_apply: the ensemble has no batched multigrid preconditioner");
+  const size_t smem = ens_smem_bytes(P);
+  CUDA_TRY(ctx, cudaFuncSetAttribute(ens_precond_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LAUNCH(ctx, ens_precond_apply_kernel, nprob, ET, smem, P, u, A, x, y);
+  CHECK_LAUNCH(ctx);
   return B200_OK;
 }

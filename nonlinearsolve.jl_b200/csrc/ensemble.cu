@@ -7,9 +7,10 @@
 //
 // Two engines:
 //   * batched (N <= 32): one CTA per trajectory, persistent over a work queue; iterate, residual, Krylov direction and the
-//     Givens recurrence live in shared memory, the Krylov basis streams through a per-CTA slab in HBM/L2.
-//     (see ens_batched.cuh)
-//   * sequential fallback (any N): the single-system driver of newton.cu, one trajectory after another.
+//     Givens recurrence live in shared memory, the Krylov basis streams through a per-CTA slab in HBM/L2; with
+//     Multigrid("left" / "right") the whole V-cycle hierarchy lives in shared memory too (see ens_batched.cu)
+//   * sequential fallback (any N): the single-system driver of newton.cu, one trajectory after another (block-Jacobi and
+//     every option set the batched kernel does not cover).
 #include "common.cuh"
 #include <algorithm>
 #include <vector>
@@ -18,6 +19,9 @@ int32_t b200i_ens_batched_supported(int32_t N, const b200_newton_opts* o);
 int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double alpha, const b200_newton_opts* o, const double* u0,
                                 const double* A, const double* B, double* u_out, double* resid_inf, int32_t* retcodes, int32_t* nsteps,
                                 int32_t* njvp, void** workspace, size_t* workspace_bytes, int32_t* n_deferred);
+int32_t b200i_ens_batched_ctas_per_sm(b200_ctx* ctx, int32_t N, const b200_newton_opts* o, int32_t* per_sm);
+int32_t b200i_ens_batched_precond_apply(b200_ctx* ctx, int32_t N, int32_t nprob, double alpha, const b200_newton_opts* o, const double* u,
+                                        const double* A, const double* x, double* y);
 
 struct b200_ensemble {
   b200_ctx* ctx;
@@ -59,9 +63,16 @@ int32_t b200_ens_destroy(b200_ensemble* e) {
 int32_t b200_ens_create(b200_ctx* ctx, int32_t N, int32_t nprob_local, double alpha, const b200_newton_opts* opts, b200_ensemble** out) {
   B200_DEVICE_GUARD(ctx);
   B200_REQUIRE(ctx, N >= 3 && nprob_local > 0 && opts && out, "ens_create: bad arguments");
-  B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_GMRES && opts->globalization == B200_GLOBALIZATION_NONE && opts->precond == B200_PRECOND_NONE &&
-                        opts->descent == B200_DESCENT_NEWTON,
+  B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_GMRES && opts->globalization == B200_GLOBALIZATION_NONE && opts->descent == B200_DESCENT_NEWTON,
                "ensemble: only matrix-free NewtonRaphson(linsolve = GMRES) trajectories are batched");
+  const int32_t pc = opts->precond;
+  B200_REQUIRE(ctx, pc != B200_PRECOND_ILU0_LEFT && pc != B200_PRECOND_ILU0_RIGHT && pc != B200_PRECOND_AMG_LEFT && pc != B200_PRECOND_AMG_RIGHT &&
+                        pc != B200_PRECOND_SA_AMG_LEFT && pc != B200_PRECOND_SA_AMG_RIGHT,
+               "ensemble: ILU0 and AMG precondition the assembled sparse Jacobian, and ensemble trajectories are matrix-free: use "
+               "Multigrid or BlockJacobi");
+  B200_REQUIRE(ctx, pc == B200_PRECOND_NONE || pc == B200_PRECOND_BLOCK_JACOBI_LEFT || pc == B200_PRECOND_BLOCK_JACOBI_RIGHT ||
+                        pc == B200_PRECOND_MULTIGRID_LEFT || pc == B200_PRECOND_MULTIGRID_RIGHT,
+               "ensemble: unknown preconditioner");
   b200_ensemble* e = new b200_ensemble();
   memset(e, 0, sizeof(*e));
   e->ctx = ctx; e->N = N; e->nprob = nprob_local; e->alpha = alpha; e->o = *opts;
@@ -150,6 +161,27 @@ int32_t b200_ens_solve(b200_ensemble* e, const double* u0, const double* A, cons
   } else {
     CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
   }
+  return B200_OK;
+}
+
+int32_t b200_ens_precond_apply(b200_ensemble* e, const double* u_dev, const double* A_dev, const double* x_dev, double* y_dev) {
+  B200_DEVICE_GUARD(e ? e->ctx : nullptr);
+  if (!e) return B200_ERR_INVALID;
+  b200_ctx* ctx = e->ctx;
+  B200_REQUIRE(ctx, u_dev && A_dev && x_dev && y_dev, "ens_precond_apply: bad arguments");
+  B200_REQUIRE(ctx, e->batched && (e->o.precond == B200_PRECOND_MULTIGRID_LEFT || e->o.precond == B200_PRECOND_MULTIGRID_RIGHT),
+               "ens_precond_apply: only a batched multigrid ensemble applies its preconditioner");
+  B200_TRY(b200i_ens_batched_precond_apply(ctx, e->N, e->nprob, e->alpha, &e->o, u_dev, A_dev, x_dev, y_dev));
+  CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));
+  return B200_OK;
+}
+
+int32_t b200_ens_ctas_per_sm(b200_ensemble* e, int32_t* ctas_per_sm) {
+  B200_DEVICE_GUARD(e ? e->ctx : nullptr);
+  if (!e) return B200_ERR_INVALID;
+  B200_REQUIRE(e->ctx, ctas_per_sm, "ens_ctas_per_sm: bad arguments");
+  *ctas_per_sm = 0;
+  if (e->batched) B200_TRY(b200i_ens_batched_ctas_per_sm(e->ctx, e->N, &e->o, ctas_per_sm));
   return B200_OK;
 }
 }  // extern "C"

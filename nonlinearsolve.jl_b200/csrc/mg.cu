@@ -14,6 +14,7 @@
 // preconditioning of plain GMRES.  Everything is elementwise / stencil work on data that is tiny next to the Krylov basis:
 // one kernel family (`mg_op_kernel`), HBM-bound, ~5 fine-grid stencil sweeps per application.
 #include "common.cuh"
+#include "mg_cell.cuh"
 #include <math.h>
 #include <vector>
 
@@ -29,21 +30,6 @@ struct MgLevel {
   double *x, *x2, *b, *r;  // 2 NC each (level 0: b and the result are the caller's vectors)
 };
 
-__device__ __forceinline__ void cell_coords(int64_t c, int N, int dim, int& i, int& j, int& k) {
-  if (dim == 3) {
-    const int64_t N2 = (int64_t)N * N;
-    k = (int)(c / N2);
-    const int r = (int)(c - (int64_t)k * N2);
-    j = r / N;
-    i = r - j * N;
-  } else {
-    k = 0;
-    j = (int)(c / N);
-    i = (int)(c - (int64_t)j * N);
-  }
-}
-__device__ __forceinline__ int wrap(int i, int N) { return i < 0 ? i + N : (i >= N ? i - N : i); }
-
 // MODE 0: out = A x ; 1: out = b - A x ; 2: out = x + omega D^-1 (b - A x) ; 3: out = omega D^-1 b  (x == 0)
 template <int MODE>
 __global__ void __launch_bounds__(MG_THREADS) mg_op_kernel(int N, int dim, int64_t NC, double a, double A, const double* __restrict__ state,
@@ -51,104 +37,24 @@ __global__ void __launch_bounds__(MG_THREADS) mg_op_kernel(int N, int dim, int64
                                                             double omega) {
   const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= NC) return;
-  const double uc = state[c], vc = state[c + NC];
-  const double uv2 = 2.0 * uc * vc, uu = uc * uc;
-  const double lapd = -2.0 * dim * a;
-  const double d00 = lapd + (uv2 - (A + 1.0)), d01 = uu, d10 = A - uv2, d11 = lapd - uu;
-  double r0, r1;
-  if (MODE == 3) {
-    r0 = b[c]; r1 = b[c + NC];
-  } else {
-    int i, j, k;
-    cell_coords(c, N, dim, i, j, k);
-    const int64_t N2 = (int64_t)N * N;
-    const int64_t base = c - i;                   // start of the i-line
-    const int64_t cim = base + wrap(i - 1, N), cip = base + wrap(i + 1, N);
-    const int64_t jb = c - (int64_t)j * N;        // same (i, k), j = 0
-    const int64_t cjm = jb + (int64_t)wrap(j - 1, N) * N, cjp = jb + (int64_t)wrap(j + 1, N) * N;
-    const double x0 = x[c], x1 = x[c + NC];
-    double l0 = x[cim] + x[cip] + x[cjp] + x[cjm] - 4.0 * x0;
-    double l1 = x[cim + NC] + x[cip + NC] + x[cjp + NC] + x[cjm + NC] - 4.0 * x1;
-    if (dim == 3) {
-      const int64_t kb = c - (int64_t)k * N2;
-      const int64_t ckm = kb + (int64_t)wrap(k - 1, N) * N2, ckp = kb + (int64_t)wrap(k + 1, N) * N2;
-      l0 = l0 + (x[ckp] + x[ckm] - 2.0 * x0);
-      l1 = l1 + (x[ckp + NC] + x[ckm + NC] - 2.0 * x1);
-    }
-    const double y0 = a * l0 + (uv2 - (A + 1.0)) * x0 + uu * x1;   // same expression order as the problem's exact JVP
-    const double y1 = a * l1 + (A - uv2) * x0 - uu * x1;
-    if (MODE == 0) { out[c] = y0; out[c + NC] = y1; return; }
-    r0 = b[c] - y0; r1 = b[c + NC] - y1;
-    if (MODE == 1) { out[c] = r0; out[c + NC] = r1; return; }
-  }
-  const double det = d00 * d11 - d01 * d10;
-  const double e0 = (d11 * r0 - d01 * r1) / det, e1 = (d00 * r1 - d10 * r0) / det;
-  if (MODE == 3) { out[c] = omega * e0; out[c + NC] = omega * e1; }
-  else { out[c] = x[c] + omega * e0; out[c + NC] = x[c + NC] + omega * e1; }
+  mg_op_cell<MODE>(c, N, dim, NC, a, A, state, x, b, out, omega);
 }
 
-// Vertex-centred transfers for any integer ratio r (coarse point I sits on fine point r I):
-//   prolongation  fine[r I + d] = (1 - d/r) c[I] + (d/r) c[I + 1] per direction (multilinear)
-//   restriction   R = P' / r^dim: coarse[I] = sum_{|d| < r} (1 - |d|/r)/r * fine[r I + d] per direction (r = 2: 1/4, 1/2, 1/4)
-// Both species.  One thread per coarse (restrict) / fine (prolong) cell; the coarse grids are tiny next to the fine one.
+// Transfers (mg_cell.cuh): one thread per coarse (restrict) / fine (prolong) cell; the coarse grids are tiny next to the fine one.
 __global__ void __launch_bounds__(MG_THREADS) mg_restrict_kernel(int Nf, int Nc, int dim, int ratio, const double* __restrict__ fine,
                                                                   double* __restrict__ coarse) {
   const int64_t NCc = dim == 3 ? (int64_t)Nc * Nc * Nc : (int64_t)Nc * Nc;
-  const int64_t NCf = dim == 3 ? (int64_t)Nf * Nf * Nf : (int64_t)Nf * Nf;
   const int64_t C = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (C >= NCc) return;
-  int I, J, K;
-  cell_coords(C, Nc, dim, I, J, K);
-  double s0 = 0.0, s1 = 0.0;
-  const int hi = ratio - 1;
-  const int khi = dim == 3 ? hi : 0;
-  const double rinv = 1.0 / ratio;
-  for (int dk = -khi; dk <= khi; ++dk) {
-    const double wk = dim == 3 ? (1.0 - abs(dk) * rinv) * rinv : 1.0;
-    const int fk = dim == 3 ? wrap(ratio * K + dk, Nf) : 0;
-    for (int dj = -hi; dj <= hi; ++dj) {
-      const double wj = (1.0 - abs(dj) * rinv) * rinv;
-      const int fj = wrap(ratio * J + dj, Nf);
-      for (int di = -hi; di <= hi; ++di) {
-        const double w = wk * wj * ((1.0 - abs(di) * rinv) * rinv);
-        const int fi = wrap(ratio * I + di, Nf);
-        const int64_t f = fi + (int64_t)Nf * (fj + (int64_t)Nf * fk);
-        s0 += w * fine[f];
-        s1 += w * fine[f + NCf];
-      }
-    }
-  }
-  coarse[C] = s0;
-  coarse[C + NCc] = s1;
+  mg_restrict_cell(C, Nf, Nc, dim, ratio, fine, coarse);
 }
 
 __global__ void __launch_bounds__(MG_THREADS) mg_prolong_add_kernel(int Nf, int Nc, int dim, int ratio, const double* __restrict__ coarse,
                                                                      double* __restrict__ fine) {
-  const int64_t NCc = dim == 3 ? (int64_t)Nc * Nc * Nc : (int64_t)Nc * Nc;
   const int64_t NCf = dim == 3 ? (int64_t)Nf * Nf * Nf : (int64_t)Nf * Nf;
   const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= NCf) return;
-  int i, j, k;
-  cell_coords(f, Nf, dim, i, j, k);
-  const double rinv = 1.0 / ratio;
-  const int I0 = i / ratio, J0 = j / ratio, K0 = k / ratio;
-  const int di = i - I0 * ratio, dj = j - J0 * ratio, dk = k - K0 * ratio;
-  const int ni = di ? 2 : 1, nj = dj ? 2 : 1, nk = (dim == 3 && dk) ? 2 : 1;
-  double s0 = 0.0, s1 = 0.0;
-  for (int ck = 0; ck < nk; ++ck) {
-    const double wk = dim == 3 ? (ck ? dk * rinv : 1.0 - dk * rinv) : 1.0;
-    for (int cj = 0; cj < nj; ++cj) {
-      const double wj = cj ? dj * rinv : 1.0 - dj * rinv;
-      for (int ci = 0; ci < ni; ++ci) {
-        const double w = wk * wj * (ci ? di * rinv : 1.0 - di * rinv);
-        const int64_t C = wrap(I0 + ci, Nc) + (int64_t)Nc * (wrap(J0 + cj, Nc) + (int64_t)Nc * (dim == 3 ? wrap(K0 + ck, Nc) : 0));
-        s0 += w * coarse[C];
-        s1 += w * coarse[C + NCc];
-      }
-    }
-  }
-  fine[f] += s0;
-  fine[f + NCf] += s1;
+  mg_prolong_add_cell(f, Nf, Nc, dim, ratio, coarse, fine);
 }
 
 inline int mg_grid(int64_t n) { return (int)((n + MG_THREADS - 1) / MG_THREADS); }
@@ -156,8 +62,9 @@ inline int mg_grid(int64_t n) { return (int)((n + MG_THREADS - 1) / MG_THREADS);
 
 struct b200_mg {
   b200_ctx* ctx;
+  const b200_problem* prob;  // the problem whose Jacobian this approximates: its A is read at every setup (b200_problem_set_AB)
   int dim, nlev;
-  double A;
+  double A;                  // the reaction parameter of the current linearisation point
   double omega;
   MgLevel lev[MG_MAX_LEVELS];
   std::vector<double*> owned;
@@ -220,7 +127,7 @@ int32_t b200i_mg_create(b200_problem* prob, b200_mg** out) {
   b200_ctx* ctx = prob->ctx;
   B200_REQUIRE(ctx, prob->kind == B200_PROB_BRUSS2D || prob->kind == B200_PROB_BRUSS3D, "multigrid preconditioner: built-in Brusselator problems only");
   b200_mg* mg = new b200_mg();
-  mg->ctx = ctx; mg->dim = prob->kind == B200_PROB_BRUSS3D ? 3 : 2; mg->A = prob->A; mg->omega = 0.8; mg->nlev = 0;
+  mg->ctx = ctx; mg->prob = prob; mg->dim = prob->kind == B200_PROB_BRUSS3D ? 3 : 2; mg->A = prob->A; mg->omega = 0.8; mg->nlev = 0;
   int N = prob->N;
   double a = prob->a;
   for (;;) {
@@ -262,9 +169,11 @@ int32_t b200i_mg_destroy(b200_mg* mg) {
 }
 
 // (re)build the coarse operators for the linearisation point u: restrict the state level by level (the same transfer as the
-// residuals), a_l is fixed by the geometry.  Called once per Newton step, like update_A! rebuilds Pl / Pr.
+// residuals), a_l is fixed by the geometry, A is the problem's current one (it changes under b200_problem_set_AB: reinit with new
+// parameters, or the ensemble's per-trajectory route).  Called once per Newton step, like update_A! rebuilds Pl / Pr.
 int32_t b200i_mg_setup(b200_mg* mg, const double* u) {
   b200_ctx* ctx = mg->ctx;
+  mg->A = mg->prob->A;
   mg->lev[0].state = const_cast<double*>(u);
   for (int l = 0; l + 1 < mg->nlev; ++l) {
     MgLevel &L = mg->lev[l], &Cl = mg->lev[l + 1];
