@@ -127,6 +127,7 @@ enum { B200_TERM_ABS_NORM_SAFE_BEST = 0, B200_TERM_ABS_NORM = 1, B200_TERM_ABS_N
 enum { B200_NORM_INF = 0, B200_NORM_L2 = 1 }; /* internalnorm: maximum(abs, .) (NonlinearProblem default) or norm(., 2) */
 enum { B200_U0_REFERENCE = 0, B200_U0_PERTURBED_Z = 1 };
 enum { B200_ORDER_NATURAL = 0, B200_ORDER_LARGEST_FIRST = 1 };
+enum { B200_STENCIL_RESIDUAL = 0, B200_STENCIL_RESIDUAL_NORM = 1, B200_STENCIL_JVP = 2, B200_STENCIL_VJP = 3 }; /* b200_problem_stencil_plan */
 
 typedef struct b200_ctx b200_ctx;
 typedef struct b200_problem b200_problem;
@@ -305,6 +306,11 @@ int32_t b200_jvp(b200_problem* prob, const double* u, const double* v, double* J
 int32_t b200_residual_jvp(b200_problem* prob, const double* u, const double* v, double* du, double* Jv); /* one halo load */
 int32_t b200_jvp_fd(b200_problem* prob, const double* u, const double* v, double* Jv);                   /* (f(u+eps v)-f(u))/eps, fused */
 int32_t b200_vjp(b200_problem* prob, const double* u, const double* w, double* JTw);
+/* the residual with the fused maximum(abs, f) epilogue the Newton driver uses; non-finite entries give +inf */
+int32_t b200_residual_norminf(b200_problem* prob, const double* u, double* du, double* norm_host);
+/* how a Brusselator op (B200_STENCIL_*) launches on this context: ring_slots = 0 is the thread-per-cell kernel, else the depth of
+   the 3D halo ring; grid = CTAs; max_marches = the most plane-chunk marches any ring CTA makes (0 for the plain kernel) */
+int32_t b200_problem_stencil_plan(b200_problem* prob, int32_t op, int32_t* ring_slots, int32_t* grid, int32_t* max_marches);
 
 /* ---------------------------------------------------------------- linear operators + GMRES (a3) */
 int32_t b200_linop_from_problem(b200_problem* prob, const double* u, int32_t jvp_mode, b200_linop** op);

@@ -39,6 +39,7 @@ TERM_ABS_NORM_SAFE_BEST, TERM_ABS_NORM, TERM_ABS_NORM_SAFE, TERM_NORM, TERM_REL,
 NORM_INF, NORM_L2 = 0, 1
 U0_REFERENCE, U0_PERTURBED_Z = 0, 1
 ORDER_NATURAL, ORDER_LARGEST_FIRST = 0, 1
+STENCIL_RESIDUAL, STENCIL_RESIDUAL_NORM, STENCIL_JVP, STENCIL_VJP = 0, 1, 2, 3
 KID_NAMES = ["jvp", "multidot", "update", "mgs", "normalize", "residual", "givens", "resident", "lu_panel", "lu_gemm", "lu_other", "sparse"]
 
 
@@ -158,6 +159,8 @@ SIGNATURES = {
     "b200_residual_jvp": (I32, [P, P, P, P, P]),
     "b200_jvp_fd": (I32, [P, P, P, P]),
     "b200_vjp": (I32, [P, P, P, P]),
+    "b200_residual_norminf": (I32, [P, P, P, PF64]),
+    "b200_problem_stencil_plan": (I32, [P, I32, PI32, PI32, PI32]),
     "b200_linop_from_problem": (I32, [P, P, I32, PP]),
     "b200_linop_from_csc": (I32, [P, I64, P, P, P, I32, PP]),
     "b200_linop_from_dense": (I32, [P, I64, P, I64, PP]),

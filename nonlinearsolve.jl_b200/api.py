@@ -1008,6 +1008,19 @@ class _DeviceProblem:
         check(self.ctx.handle, lib().b200_residual_jvp(self._h, u.ptr, v.ptr, du.ptr, Jv.ptr))
         return du, Jv
 
+    def residual_norminf(self, u, du=None):
+        """(f(u), maximum(abs, f(u))) through the residual kernel's fused norm epilogue (non-finite entries give +inf)."""
+        du = du or self.ctx.empty(self.n)
+        out = C.c_double()
+        check(self.ctx.handle, lib().b200_residual_norminf(self._h, u.ptr, du.ptr, C.byref(out)))
+        return du, out.value
+
+    def stencil_plan(self, op):
+        """(ring_slots, grid, max_marches) of a Brusselator op (abi.STENCIL_*) on this context; ring_slots == 0: plain kernel."""
+        r, g, m = C.c_int32(), C.c_int32(), C.c_int32()
+        check(self.ctx.handle, lib().b200_problem_stencil_plan(self._h, int(op), C.byref(r), C.byref(g), C.byref(m)))
+        return r.value, g.value, m.value
+
     def u0(self, mode=abi.U0_REFERENCE):
         u = self.ctx.empty(self.n)
         check(self.ctx.handle, lib().b200_problem_u0(self._h, mode, u.ptr))

@@ -417,6 +417,36 @@ __global__ void __launch_bounds__(PB_THREADS) bruss_u0_kernel(int dim, int N, in
 
 inline int grid_for(int64_t n) { return (int)((n + PB_THREADS - 1) / PB_THREADS); }
 
+// Which Brusselator kernel an op runs and with what grid.  `tiled`: the op has a ring-kernel instantiation (residual, residual
+// + norm, JVP, VJP); `has_y`: its slots also carry the centre-only field (JVP, VJP).  ring_slots == 0 selects the plain kernel.
+struct StencilPlan {
+  int ring_slots, grid, max_marches;
+  size_t slot_bytes;
+};
+StencilPlan stencil_plan(int dim, int N, bool tiled, bool has_y, int sm_count) {
+  const int64_t NC = (dim == 2) ? (int64_t)N * N : (int64_t)N * N * N;
+  const StencilPlan plain{0, grid_for(NC), 0, 0};
+  const int N2 = N * N;
+  if (dim == 2 || !tiled || N % 2 != 0 || N2 < TS_L + 2 * N) return plain;
+  const size_t slot = sizeof(double) * (2 * (size_t)(TS_L + 2 * N) + (has_y ? 2 * TS_L : 0));
+  // two CTAs per SM share the 227 KB; the depth of the ring is not what bounds a kernel this short (a few microseconds of
+  // traffic at N = 100), so it stays at up to 8 slots
+  const int R = (int)std::min<size_t>(TS_MAXR, (size_t)(100 * 1024) / slot);
+  const int per_sm = 2;
+  const int chunks = (N2 + TS_L - 1) / TS_L;
+  const int64_t W = (int64_t)chunks * N;
+  // one wave, two CTAs per SM; every CTA gets a run of >= 2 planes and crosses at most TS_MAXMARCH - 1 chunk boundaries
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(per_sm * (int64_t)sm_count, W / 2));
+  if (R < 4 || (W + grid - 1) / grid > (int64_t)(TS_MAXMARCH - 1) * N) return plain;
+  // CTA b marches over plane-chunks [W b / grid, W (b + 1) / grid): one march per chunk its run touches (the kernel's prologue)
+  int max_marches = 0;
+  for (int b = 0; b < grid; ++b) {
+    const int64_t w0 = W * b / grid, w1 = W * (b + 1) / grid;
+    if (w1 > w0) max_marches = std::max(max_marches, (int)((w1 - 1) / N - w0 / N + 1));
+  }
+  return StencilPlan{R, grid, max_marches, slot};
+}
+
 template <int MODE>
 int32_t launch_bruss(b200_problem* p, const double* u, const double* d, double* du, double* Jd, double* norm_out, const double* eps) {
   b200_ctx* ctx = p->ctx;
@@ -425,31 +455,20 @@ int32_t launch_bruss(b200_problem* p, const double* u, const double* d, double* 
   // algorithmic bytes: residual 2 Bv, JVP/VJP/FD-JVP 3 Bv, fused residual+JVP 4 Bv (DESIGN.md)
   const int kid = (MODE & M_RESID) && !(MODE & (M_JVP | M_VJP)) ? B200_KID_RESIDUAL : B200_KID_JVP;
   const double pbytes = 8.0 * (double)p->n * (((MODE & M_RESID) ? 2.0 : 0.0) + ((MODE & (M_JVP | M_VJP | M_FD)) ? ((MODE & M_RESID) ? 2.0 : 3.0) : 0.0));
+  constexpr bool tiled = MODE == M_RESID || MODE == (M_RESID | M_NORM) || MODE == M_JVP || MODE == M_VJP;
+  constexpr bool has_y = (MODE & (M_JVP | M_VJP)) != 0;
+  const StencilPlan pl = stencil_plan(p->kind == B200_PROB_BRUSS2D ? 2 : 3, p->N, tiled, has_y, ctx->sm_count);
   if (p->kind == B200_PROB_BRUSS2D) {
-    PLAUNCH(ctx, kid, pbytes, (bruss2d_kernel<MODE>), grid_for((int64_t)p->N * p->N), PB_THREADS, 0, P, u, d, forcing, du, Jd, norm_out, eps);
+    PLAUNCH(ctx, kid, pbytes, (bruss2d_kernel<MODE>), pl.grid, PB_THREADS, 0, P, u, d, forcing, du, Jd, norm_out, eps);
   } else {
-    constexpr bool tiled = MODE == M_RESID || MODE == (M_RESID | M_NORM) || MODE == M_JVP || MODE == M_VJP;
-    const int N = p->N, N2 = N * N;
     bool done = false;
-    if constexpr (tiled) if ((N % 2 == 0) && N2 >= TS_L + 2 * N) {
-      constexpr bool has_y = (MODE & (M_JVP | M_VJP)) != 0;
-      const size_t slot = sizeof(double) * (2 * (size_t)(TS_L + 2 * N) + (has_y ? 2 * TS_L : 0));
-      // two CTAs per SM share the 227 KB; the depth of the ring is not what bounds a kernel this short (a few microseconds of
-      // traffic at N = 100), so it stays at up to 8 slots
-      const int R = (int)std::min<size_t>(TS_MAXR, (size_t)(100 * 1024) / slot);
-      const int per_sm = 2;
-      const int chunks = (N2 + TS_L - 1) / TS_L;
-      const int64_t W = (int64_t)chunks * N;
-      // one wave, two CTAs per SM; every CTA gets a run of >= 2 planes and crosses at most TS_MAXMARCH - 1 chunk boundaries
-      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(per_sm * (int64_t)ctx->sm_count, W / 2));
-      if (R >= 4 && (W + grid - 1) / grid <= (int64_t)(TS_MAXMARCH - 1) * N) {
-        const size_t smem = slot * R;
-        CUDA_TRY(ctx, cudaFuncSetAttribute(bruss3d_ring_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        PLAUNCH(ctx, kid, pbytes, (bruss3d_ring_kernel<MODE>), grid, TS_THREADS + 32, smem, P, R, u, d, forcing, (MODE & M_RESID) ? du : Jd, norm_out);
-        done = true;
-      }
+    if constexpr (tiled) if (pl.ring_slots > 0) {
+      const size_t smem = pl.slot_bytes * pl.ring_slots;
+      CUDA_TRY(ctx, cudaFuncSetAttribute(bruss3d_ring_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      PLAUNCH(ctx, kid, pbytes, (bruss3d_ring_kernel<MODE>), pl.grid, TS_THREADS + 32, smem, P, pl.ring_slots, u, d, forcing, (MODE & M_RESID) ? du : Jd, norm_out);
+      done = true;
     }
-    if (!done) PLAUNCH(ctx, kid, pbytes, (bruss3d_kernel<MODE>), grid_for((int64_t)p->N * p->N * p->N), PB_THREADS, 0, P, u, d, forcing, du, Jd, norm_out, eps);
+    if (!done) PLAUNCH(ctx, kid, pbytes, (bruss3d_kernel<MODE>), pl.grid, PB_THREADS, 0, P, u, d, forcing, du, Jd, norm_out, eps);
   }
   CHECK_LAUNCH(ctx);
   return B200_OK;
@@ -630,6 +649,28 @@ int32_t b200_vjp(b200_problem* p, const double* u, const double* w, double* JTw)
       return ctx->fail(B200_ERR_UNSUPPORTED, "callback problem has no vjp", __FILE__, __LINE__);
   }
   return ctx->fail(B200_ERR_INVALID, "unknown problem kind", __FILE__, __LINE__);
+}
+
+int32_t b200_residual_norminf(b200_problem* p, const double* u, double* du, double* norm_host) {
+  B200_DEVICE_GUARD(p ? p->ctx : nullptr);
+  b200_ctx* ctx = p->ctx;
+  B200_REQUIRE(ctx, u && du && norm_host, "residual_norminf: bad arguments");
+  CUDA_TRY(ctx, cudaMemsetAsync(ctx->d_scalars, 0, sizeof(double), ctx->stream));
+  B200_TRY(b200i_residual_norm(p, u, du, ctx->d_scalars));
+  B200_TRY(b200i_fetch_scalars(ctx, 1));
+  *norm_host = ctx->h_scalars[0];
+  return B200_OK;
+}
+
+int32_t b200_problem_stencil_plan(b200_problem* p, int32_t op, int32_t* ring_slots, int32_t* grid, int32_t* max_marches) {
+  b200_ctx* ctx = p->ctx;
+  B200_REQUIRE(ctx, p->kind == B200_PROB_BRUSS2D || p->kind == B200_PROB_BRUSS3D, "stencil_plan: not a Brusselator problem");
+  B200_REQUIRE(ctx, op >= B200_STENCIL_RESIDUAL && op <= B200_STENCIL_VJP && ring_slots && grid && max_marches, "stencil_plan: bad arguments");
+  const StencilPlan pl = stencil_plan(p->kind == B200_PROB_BRUSS2D ? 2 : 3, p->N, true, op == B200_STENCIL_JVP || op == B200_STENCIL_VJP, ctx->sm_count);
+  *ring_slots = pl.ring_slots;
+  *grid = pl.grid;
+  *max_marches = pl.max_marches;
+  return B200_OK;
 }
 
 int32_t b200_residual_jvp(b200_problem* p, const double* u, const double* v, double* du, double* Jv) {
