@@ -200,6 +200,20 @@ __device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, 
                "l"(gsrc), "r"(bytes), "r"((unsigned)__cvta_generic_to_shared(bar))
                : "memory");
 }
+// L2 cache policy for data read once: the lines an access with this hint touches are the first candidates for eviction, so
+// streamed data does not push out what was prefetched into L2 for later.  Created at the point of use (one instruction) so
+// that no register holds it across a loop.
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// tma_bulk_load with an L2 cache policy (l2_evict_first_policy)
+__device__ __forceinline__ void tma_bulk_load(void* smem_dst, const void* gsrc, unsigned bytes, uint64_t* bar, uint64_t policy) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+               ::"r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(gsrc), "r"(bytes), "r"((unsigned)__cvta_generic_to_shared(bar)), "l"(policy)
+               : "memory");
+}
 // bulk prefetch of `bytes` (multiple of 16, 16-byte aligned) of global memory into L2; no completion to wait for
 __device__ __forceinline__ void l2_bulk_prefetch(const void* gsrc, unsigned bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
@@ -207,6 +221,11 @@ __device__ __forceinline__ void l2_bulk_prefetch(const void* gsrc, unsigned byte
 // 16-byte global -> shared copy (non-bulk cp.async, L2 only); completes into the thread's current cp.async group
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
+}
+// the same with an L2 cache policy (l2_evict_first_policy)
+__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc, uint64_t policy) {
+  asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(gsrc), "l"(policy)
+               : "memory");
 }
 // orders this thread's generic-proxy accesses to shared memory (loads, stores, completed non-bulk cp.async) before later
 // async-proxy (TMA) accesses; place it before the barrier after which one thread issues the bulk copy

@@ -607,7 +607,8 @@ struct R3Ctx {
 
 // The shared-memory stages hold the CTA's rows [0, 2 * R3_THREADS * qs): a prefix of the first species' segment, or all of it
 // and a prefix of the second species' segment.  The rows past the stage (the global tail) are prefetched into L2 here, so that
-// their copies into stage slots and the direct reads of the stage-1 dot sweep end in L2 instead of HBM.
+// their copies into stage slots and the direct reads of the stage-1 dot sweep end in L2 instead of HBM.  The copy reads
+// evict-first: the rows it copies are not needed again in this launch.
 __device__ __forceinline__ void r3_issue_smem(const ResidentParams& P, const R3Ctx& cx, uint64_t* mbar, int t, int stage) {
   if (threadIdx.x == 0 && cx.nrow > 0) {
     const double* src = P.V[t % cx.k];
@@ -615,9 +616,10 @@ __device__ __forceinline__ void r3_issue_smem(const ResidentParams& P, const R3C
     const int srow = min(cx.nrow, 2 * R3_THREADS * cx.qs);
     const int r0 = min(srow, cx.ncell), r1 = srow - r0;
     const int64_t c0 = (int64_t)cx.b * P.cpc;
+    const uint64_t pol = l2_evict_first_policy();
     mbar_expect_tx(&mbar[stage], (unsigned)srow * 8u);
-    tma_bulk_load(dst, src + c0, (unsigned)r0 * 8u, &mbar[stage]);
-    if (r1 > 0) tma_bulk_load(dst + cx.ncell, src + P.NC + c0, (unsigned)r1 * 8u, &mbar[stage]);
+    tma_bulk_load(dst, src + c0, (unsigned)r0 * 8u, &mbar[stage], pol);
+    if (r1 > 0) tma_bulk_load(dst + cx.ncell, src + P.NC + c0, (unsigned)r1 * 8u, &mbar[stage], pol);
     // rows [srow, nrow): the rest of the first species' segment, then the second species' rows from max(srow, ncell) on
     // (even bounds: every range is a multiple of 16 bytes)
     if (srow < cx.ncell) l2_bulk_prefetch(src + c0 + srow, (unsigned)(cx.ncell - srow) * 8u);
@@ -670,11 +672,17 @@ __device__ __forceinline__ bool r3_update_slot(const R3Ctx& cx, int q) { return 
 // hop as in r3_issue_regs) -> slots 0 .. nslot-1 of a stage (`ts` = the stage + 2 * tid), one cp.async group.  Every source
 // lies in this CTA's rows of one species' segment; sources and slots are 16-byte aligned (even offsets of aligned bases).
 // Call only when the thread has a tail pair (lim > 2 * R3_THREADS * qs): the group it commits is waited on in R3_SLOTGET.
+// LAST: the copy of the update sweep, the tail's last use in this launch, reads evict-first; the copy for the dot sweep
+// (LAST = false) reads with the default policy, so that the tail is still in L2 for the update sweep one step later.
+template <bool LAST = true>
 __device__ __forceinline__ void r3_tail_copy(const R3Ctx& cx, const double* gp, double* ts, int nslot, int lim, int lims, int64_t hop) {
+  const uint64_t pol = LAST ? l2_evict_first_policy() : 0;
   for (int j = 0; j < nslot; ++j) {
     const int lr = 2 * R3_THREADS * (cx.qs + j);
     if (lr >= lim) break;  // also ends the copy at pair R3_RP - 1
-    cp_async16(ts + 2 * R3_THREADS * j, gp + lr + ((lr >= lims) ? hop : (int64_t)0));
+    const double* src = gp + lr + ((lr >= lims) ? hop : (int64_t)0);
+    if (LAST) cp_async16(ts + 2 * R3_THREADS * j, src, pol);
+    else cp_async16(ts + 2 * R3_THREADS * j, src);
   }
   asm volatile("cp.async.commit_group;" ::: "memory");
 }
@@ -683,14 +691,17 @@ __device__ __forceinline__ void r3_issue_regs(const ResidentParams& P, const R3C
   const double* src = P.V[t % cx.k] + (int64_t)cx.b * P.cpc + 2 * (int)threadIdx.x;
   const int lim = cx.nrow - 2 * (int)threadIdx.x, lims = cx.ncell - 2 * (int)threadIdx.x;
   const int64_t hop = P.NC - cx.ncell;  // from the end of this CTA's first-species segment to the start of its second
+  const uint64_t pol = l2_evict_first_policy();  // the vector is read once in this launch
 #pragma unroll
   for (int q = 0; q < R3_RP; ++q) {
     const int lr = 2 * R3_THREADS * q;
     const double* p = src + ((lr >= lims) ? hop : (int64_t)0) + lr;
     if (q < R3_RPR) {
-      if (lr < lim) asm volatile("ld.global.nc.L1::no_allocate.v2.f64 {%0, %1}, [%2];" : "=d"(vr[2 * (q < R3_RPR ? q : 0)]), "=d"(vr[2 * (q < R3_RPR ? q : 0) + 1]) : "l"(p));
+      if (lr < lim)
+        asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;"
+                     : "=d"(vr[2 * (q < R3_RPR ? q : 0)]), "=d"(vr[2 * (q < R3_RPR ? q : 0) + 1]) : "l"(p), "l"(pol));
     } else if (lr < lim) {
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(cx.annex + (q - R3_RPR) * R3_THREADS + threadIdx.x)), "l"(p) : "memory");
+      cp_async16(cx.annex + (q - R3_RPR) * R3_THREADS + threadIdx.x, p, pol);
     }
   }
   asm volatile("cp.async.commit_group;" ::: "memory");
@@ -947,7 +958,7 @@ __device__ __forceinline__ void r3g_step(const ResidentParams& P, R3Ctx& cx, R3G
     }
   } else if (ROLE == 1) {  // stage 1 is refilled after the next dot sweep; until then its slots take the tail of v_{t+2}
     if (t + 3 < cx.total) r3_prefetch_l2(P, cx, t + 3);
-    if (t + 2 < cx.total && tail) r3_tail_copy(cx, P.V[(t + 2) % cx.k] + (int64_t)cx.b * P.cpc + 2 * tid, sc, cx.qs, lim, lims, hop);
+    if (t + 2 < cx.total && tail) r3_tail_copy<false>(cx, P.V[(t + 2) % cx.k] + (int64_t)cx.b * P.cpc + 2 * tid, sc, cx.qs, lim, lims, hop);
   } else if (t + 3 < cx.total) {
     r3_issue_regs(P, cx, t + 3, vr);
   }
