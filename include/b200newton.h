@@ -464,10 +464,12 @@ int32_t b200_newton_solve_host(b200_newton* nw, const double* u0_host, double* u
                                b200_newton_result* result_host);
 
 /* ---------------------------------------------------------------- ensemble (a11): K independent 2D Brusselators
- * Trajectories are matrix-free NewtonRaphson solves with GMRES.  The preconditioner may be none, block-Jacobi or multigrid
- * (either side); ILU0 and AMG need the assembled sparse Jacobian and are refused with B200_ERR_INVALID.  For N <= 32 one kernel
- * solves the whole batch, one CTA per trajectory, with the multigrid V-cycle in shared memory; block-Jacobi, N > 32 and the
- * option sets that kernel does not cover run the single-system driver, one trajectory after another. */
+ * Trajectories are matrix-free Newton solves with GMRES: NewtonRaphson, NewtonRaphson with BackTracking, or TrustRegion
+ * (Dogleg).  The preconditioner may be none, block-Jacobi or multigrid (either side); ILU0 and AMG need the assembled sparse
+ * Jacobian and are refused with B200_ERR_INVALID, and so is a globalised (TrustRegion, BackTracking) ensemble with any
+ * preconditioner.  For N <= 32 one kernel solves the whole batch, one CTA per trajectory, with the multigrid V-cycle in shared
+ * memory or the globalisation in the same CTA; block-Jacobi, N > 32, the Bastin radius scheme and the option sets that kernel
+ * does not cover run the single-system driver, one trajectory after another. */
 typedef struct b200_ens_result {
   int32_t nprob;
   int32_t nsuccess;

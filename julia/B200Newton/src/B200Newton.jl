@@ -688,7 +688,9 @@ end
 
 `solve(ensembleprob, alg, EnsembleB200(); trajectories)` evaluates `prob_func(prob, i, repeat)` for the trajectories of
 this rank's contiguous block, packs `u0` / `(A, B)` into batches and calls `b200_ens_solve` (one CTA per trajectory, no
-collective on the data path).  With `world_size > 1` (one process per GPU) the solutions of all ranks are collected in
+collective on the data path).  `alg`'s `NewtonOpts.globalization` is forwarded: undamped Newton, the BackTracking line search
+and the trust region (Dogleg) are batched, the latter two without a preconditioner (`b200_ens_create` refuses a globalised
+ensemble with one).  With `world_size > 1` (one process per GPU) the solutions of all ranks are collected in
 trajectory order by `b200_ens_allgather` and the status counters by `b200_ens_allreduce_stats` — NCCL over NVLink inside
 the library; `unique_id` is the 128-byte id from `nccl_unique_id()` on rank 0, shipped by the launcher (MPI.bcast, a file).
 """

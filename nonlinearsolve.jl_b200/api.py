@@ -1307,8 +1307,10 @@ def shard_range(K, rank, world_size):
 class EnsembleCache:
     """Persistent per-GPU batch workspace for K_local 2D-Brusselator trajectories.  The options are those of a single solve,
     preconditioner included (`Multigrid` on either side is batched, `BlockJacobi` runs trajectory by trajectory; ILU0 and the
-    AMGs need an assembled Jacobian and are refused); option sets the batched kernel does not implement (see
-    csrc/ens_batched.cu) run each trajectory through the general driver."""
+    AMGs need an assembled Jacobian and are refused).  `alg` is `NewtonRaphson(linsolve = KrylovJL_GMRES(...))`, with or
+    without `linesearch = BackTracking()`, or `TrustRegion(linsolve = KrylovJL_GMRES(...))`; the globalised ones take no
+    preconditioner (refused otherwise), and the Bastin radius scheme runs trajectory by trajectory.  Option sets the batched
+    kernel does not implement (see csrc/ens_batched.cu) run each trajectory through the general driver."""
 
     def __init__(self, ctx, N, nprob_local, alpha, alg, abstol=None, reltol=None, maxiters=1000, termination_condition=None, maxtime=None):
         self.ctx, self.N, self.K, self.n = ctx, N, nprob_local, 2 * N * N

@@ -8,11 +8,13 @@
 //
 // Option sets batched here (b200i_ens_batched_supported): exact JVP; unrestarted GMRES with MGS or CGS2 (MGS applied twice),
 // any itmax / atol / rtol, optional EW forcing; no preconditioner, or the multigrid V-cycle of mg.cu on either side
-// (Multigrid("left") / Multigrid("right")); termination AbsNorm, AbsNormSafe or AbsNormSafeBest on the inf-norm with the
-// default step-stall window (32); no maxtime; N <= 32.  Every other option set (block-Jacobi, the Norm / Rel / Abs modes, the
-// L2 norm, another stall window, one-pass CGS, a wall-clock limit, FD-JVP, warm start, restart, N > 32) runs each trajectory
-// through the general driver of newton.cu instead (b200_ens_solve).  tests/test_gpu_ensemble.py and
-// tests/test_gpu_ensemble_precond.py check both routes.
+// (Multigrid("left") / Multigrid("right")); without a preconditioner also TrustRegion (Dogleg) with the Simple, NLsolve,
+// NocedalWright, Hei, Yuan or Fan radius scheme, and NewtonRaphson with BackTracking; termination AbsNorm, AbsNormSafe or
+// AbsNormSafeBest on the inf-norm with the default step-stall window (32); no maxtime; N <= 32.  Every other option set
+// (block-Jacobi, the Bastin scheme, the Norm / Rel / Abs modes, the L2 norm, another stall window, one-pass CGS, a wall-clock
+// limit, FD-JVP, warm start, restart, N > 32) runs each trajectory through the general driver of newton.cu instead
+// (b200_ens_solve).  tests/test_gpu_ensemble.py, tests/test_gpu_ensemble_precond.py and tests/test_gpu_ensemble_globalized.py
+// check both routes.
 //
 // Design: a 2D N=32 trajectory has n = 2048 unknowns = 16 KB per vector, so a CTA owns a whole trajectory:
 //   * iterate u and the current Krylov direction v_k live in shared memory (stencil neighbourhoods are read from there),
@@ -34,6 +36,15 @@
 // follows the driver (Krylov.jl gmres!(; M, N, ldiv = false)): right w = J M^-1 v_k and x = M^-1 V_k y; left r0 = M^-1 f,
 // w = M^-1 J v_k, the tolerance atol + rtol ||M^-1 f|| while Eisenstat-Walker keeps ||f||_2.  V-cycles are not matvecs:
 // njvp counts Arnoldi steps, as the driver's does.
+//
+// Globalisation (ens_newton_kernel<ENS_PC_NONE, ENS_GL_TRUST_REGION / ENS_GL_LINESEARCH>), after GMRES has formed x, as
+// newton.cu's dogleg / trust_region_step / backtracking do it, with the same scalars: the trust region forms J' f (ens_vjp), the
+// Cauchy direction's ||J du_c||^2 when the Newton step leaves the radius, ||J du||^2 unless the step is the cut Cauchy direction,
+// and f at the trial point; a rejected step keeps u and f and the next step runs GMRES again at the same u.  BackTracking
+// forms <f, J du> by one JVP and f at each trial point.  No shared-memory buffer is added: vk (free after GMRES) holds the
+// vector a stencil pass reads and the trial state; the first two basis columns of the slab (dead once x is formed) hold the
+// step and f; the radius state waits out GMRES in ENS_GL_STATE doubles at the head of the slab.  Every decision is taken by
+// every thread from block-reduced values.
 #include "common.cuh"
 #include "mg_cell.cuh"
 #include <algorithm>
@@ -45,6 +56,8 @@ constexpr int ENS_LS_BASIS_FULL = 100;  // internal GMRES stop code: the per-CTA
 constexpr int ET = 256;   // threads per CTA
 constexpr int NPT = 8;    // max rows per thread  -> n <= 2048 (N <= 32)
 constexpr int ENS_PC_NONE = 0, ENS_PC_MG_LEFT = 1, ENS_PC_MG_RIGHT = 2;  // preconditioner of a kernel instantiation
+constexpr int ENS_GL_NONE = 0, ENS_GL_TRUST_REGION = 1, ENS_GL_LINESEARCH = 2;  // globalisation of a kernel instantiation
+constexpr int ENS_GL_STATE = 8;  // doubles of per-trajectory globalisation state at the head of a globalised kernel's slab
 constexpr int ENS_MG_MAXLEV = 8;   // 2D N <= 32: at most 32 -> 16 -> 8 -> 4 -> 2 -> 1
 constexpr double ENS_MG_OMEGA = 0.8;
 
@@ -65,6 +78,15 @@ struct EnsParams {
   int mg_nlev, mg_tab;             // multigrid: number of levels, offset (doubles) of the level table in shared memory
   int mg_doubles;                  // multigrid: shared-memory doubles of the table and every level's buffers
   EnsMgLevel mg[ENS_MG_MAXLEV];
+};
+
+// Globalisation constants: the trust region's scheme, radii and TrParams, BackTracking's constants.  They follow every other
+// kernel parameter (the last argument of ens_newton_kernel), so no parameter the unglobalised instantiations read moves.
+struct EnsGlob {
+  int scheme, max_shrink, ls_maxiters;
+  double max_tr, init_tr;  // TrustRegion(max_trust_radius, initial_trust_radius); 0: the scheme's default
+  double step_thr, shrink_thr, expand_thr, shrink_fac, expand_fac, tp1, tp2, tp3, tp4;
+  double ls_c1, ls_rho_hi, ls_rho_lo;
 };
 
 struct CtaState {  // shared-memory scalars, written by thread 0, read after a barrier
@@ -90,6 +112,18 @@ __device__ __forceinline__ double blk_max_all(double v, double (*red)[ET / 32], 
   if ((threadIdx.x & 31) == 0) buf[threadIdx.x >> 5] = v;
   __syncthreads();
   double s = 0.0;
+#pragma unroll
+  for (int q = 0; q < ET / 32; ++q) s = fmax(s, buf[q]);
+  phase++;
+  return s;
+}
+// block maximum of values of either sign (blk_max_all starts from 0: it serves norms)
+__device__ __forceinline__ double blk_max_signed(double v, double (*red)[ET / 32], int& phase) {
+  v = warp_max(v);
+  double* buf = red[phase & 1];
+  if ((threadIdx.x & 31) == 0) buf[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = -INFINITY;
 #pragma unroll
   for (int q = 0; q < ET / 32; ++q) s = fmax(s, buf[q]);
   phase++;
@@ -164,6 +198,40 @@ __device__ __forceinline__ void ens_jvp(const EnsParams& P, double A, const doub
       w[q] = s ? (P.a * lap + (A - uv2) * dc - uu * ec) : (P.a * lap + (uv2 - (A + 1.0)) * dc + uu * ec);
     }
   }
+}
+// J^T w rows of this thread: w in shared memory, state u in shared memory.  The periodic 5-point Laplacian is symmetric; the
+// per-cell reaction block [[2uv - (A+1), u^2], [A - 2uv, -u^2]] of ens_jvp enters transposed.
+__device__ __forceinline__ void ens_vjp(const EnsParams& P, double A, const double* __restrict__ us, const double* __restrict__ ws,
+                                        double (&g)[NPT]) {
+  const int N = P.N, NC = N * N;
+  ENS_ROW_WALK_BEGIN(P, N, NC)
+#pragma unroll
+  for (int q = 0; q < NPT; ++q) {
+    const int r = threadIdx.x + ET * q;
+    g[q] = 0.0;
+    ENS_ROW_WALK_STEP(q, N)
+    if (r < P.n) {
+      const int s = rw_s, c = r - s * NC;
+      const int i = rw_i, j = rw_j;
+      const int ip = (i + 1 == N) ? 0 : i + 1, im = (i == 0) ? N - 1 : i - 1;
+      const int jp = (j + 1 == N) ? 0 : j + 1, jm = (j == 0) ? N - 1 : j - 1;
+      const double* x = ws + s * NC;
+      const double lap = x[im + N * j] + x[ip + N * j] + x[i + N * jp] + x[i + N * jm] - 4.0 * x[c];
+      const double uc = us[c], vc = us[c + NC], dc = ws[c], ec = ws[c + NC];
+      const double uv2 = 2.0 * uc * vc, uu = uc * uc;
+      g[q] = s ? (P.a * lap + uu * dc - uu * ec) : (P.a * lap + (uv2 - (A + 1.0)) * dc + (A - uv2) * ec);
+    }
+  }
+}
+
+// this thread's rows of an n-vector: to / from memory it alone touches at these rows (shared memory or the HBM slab)
+__device__ __forceinline__ void ens_put(double* dst, const double (&v)[NPT], int n) {
+#pragma unroll
+  for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) dst[r] = v[q]; }
+}
+__device__ __forceinline__ void ens_get(const double* src, double (&v)[NPT], int n) {
+#pragma unroll
+  for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; v[q] = (r < n) ? src[r] : 0.0; }
 }
 
 // ---- the multigrid V-cycle of mg.cu on one CTA, every level in shared memory
@@ -240,12 +308,13 @@ __device__ __forceinline__ void ens_mg_load_table(const EnsParams& P, EnsMgLevel
     if ((int)threadIdx.x == l) mgl[l] = P.mg[l];
 }
 
-template <int PC>
+template <int PC, int GL>
 __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const double* __restrict__ u0, const double* __restrict__ Aarr,
                                                             const double* __restrict__ Barr, const double* __restrict__ forcing,
                                                             double* __restrict__ u_out, double* __restrict__ resid_inf,
                                                             int32_t* __restrict__ retcodes, int32_t* __restrict__ nsteps_out,
-                                                            int32_t* __restrict__ njvp_out, double* __restrict__ ws, int* __restrict__ counter) {
+                                                            int32_t* __restrict__ njvp_out, double* __restrict__ ws, int* __restrict__ counter,
+                                                            EnsGlob G) {
   extern __shared__ double sm[];
   double* us = sm;                    // iterate u            [npad]
   double* vk = us + P.npad;           // current direction    [npad]
@@ -263,6 +332,10 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
   int phase = 0;
   const int n = P.n;
   double* slab = ws + (int64_t)blockIdx.x * P.slab;
+  // a globalised kernel keeps ENS_GL_STATE doubles in front of the basis: the trust region's radius, its clamp, the scheme
+  // parameter p1 (Yuan and Fan move it) and the shrink counter wait out GMRES there rather than in registers (written by
+  // thread 0, read by all after a barrier; addressed from Vg with a constant offset)
+  if constexpr (GL != ENS_GL_NONE) slab += ENS_GL_STATE;
   double* Vg = slab;                                   // (kcap + 1) vectors of npad doubles
   double* Rg = slab + (int64_t)(P.kcap + 1) * P.npad;  // packed upper triangular, column k (1-based) at (k-1)k/2
 
@@ -285,6 +358,39 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
     for (int q = 0; q < NPT; ++q) fmx = fmax(fmx, abs_nf(f[q]));
     double objective = blk_max_all(fmx, red, phase);
     double best = objective;
+    if constexpr (GL == ENS_GL_TRUST_REGION) {  // initial radius (newton.cu b200_newton_reinit; trust_region.jl:204-258, 330-346)
+      double* trs = Vg - ENS_GL_STATE;
+      // like every scalar decision of the globalisations, computed by every thread from block-reduced values
+      double tr, tr_max;
+      const double tp1 = G.tp1;
+      double fsq0 = 0.0, usq = 0.0, umx = -INFINITY, umn = -INFINITY;
+#pragma unroll
+      for (int q = 0; q < NPT; ++q) {
+        const int r = threadIdx.x + ET * q;
+        fsq0 = fma(f[q], f[q], fsq0);
+        if (r < n) { const double v = us[r]; usq = fma(v, v, usq); umx = fmax(umx, v); umn = fmax(umn, -v); }
+      }
+      const double fn0 = sqrt(blk_sum_all(fsq0, red, phase)), un0 = sqrt(blk_sum_all(usq, red, phase));
+      const double urange = blk_max_signed(umx, red, phase) + blk_max_signed(umn, red, phase);  // max u - min u
+      const int sch = G.scheme;
+      tr_max = G.max_tr > 0 ? G.max_tr : (sch == B200_TR_SIMPLE || sch == B200_TR_NOCEDAL_WRIGHT) ? (fn0 < urange ? urange : fn0) : INFINITY;
+      if (G.init_tr > 0) tr = G.init_tr;
+      else if (sch == B200_TR_NLSOLVE) tr = un0 > 0 ? un0 : 1.0;
+      else if (sch == B200_TR_HEI) tr = 1.0;
+      else if (sch == B200_TR_FAN) tr = pow(fn0, 0.99) / 10.0;
+      else tr = tr_max / 11.0;
+      if (sch == B200_TR_YUAN) {  // p1 ||J' f0||
+        ens_put(vk, f, n);
+        __syncthreads();
+        double g[NPT];
+        ens_vjp(P, A, us, vk, g);
+        double gsq = 0.0;
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) gsq = fma(g[q], g[q], gsq);
+        tr = tp1 * sqrt(blk_sum_all(gsq, red, phase));
+      }
+      if (threadIdx.x == 0) { trs[0] = tr; trs[1] = tr_max; trs[2] = tp1; trs[3] = 0.0; }
+    }
     int retcode = B200_RC_DEFAULT, nsteps = 0, njvp = 0, tc_nsteps = 0, force_stop = 0;
     bool rolled_back_needed = false;
     double eta = P.ew_eta0, rnorm_nl = 0.0, rnorm_nl_prev = 0.0;
@@ -452,7 +558,11 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
         }
       }
       // ================= u += du, du = -x ; fu = f(u) ; termination (solve.jl:436-452) =================
+      // a globalised step leaves this thread's part of ||du||_2^2 in dsq (0 for a rejected trust-region step) and the new
+      // ||f||_inf in objective; glob_rc is its own stop (shrink limit, failed line search), behind the termination test
       double dsq = 0.0;
+      int glob_rc = 0;
+      if constexpr (GL == ENS_GL_NONE) {
       __syncthreads();
 #pragma unroll
       for (int q = 0; q < NPT; ++q) {
@@ -465,6 +575,224 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
 #pragma unroll
       for (int q = 0; q < NPT; ++q) fmx = fmax(fmx, abs_nf(f[q]));
       objective = blk_max_all(fmx, red, phase);
+      } else if constexpr (GL == ENS_GL_TRUST_REGION) {
+        // ================= Dogleg (newton.cu dogleg; dogleg.jl:86-151) =================
+        // vk is free once GMRES is done and the basis slab once x is formed.  vk holds the vector a VJP / JVP reads, then the
+        // trial state; slab column 0 the step du, then f(u_trial); column 1 the residual f.  Each thread touches only its own
+        // rows of the slab, so those need no barrier.  f is not kept in registers through GMRES: it is evaluated again here, to
+        // the same bits.  J' f is formed first: the ratio needs it, and the Cauchy direction is du_c = -J' f (steepest.jl:60-80).
+        // The step has one VJP and one JVP site (the JVP in a two-pass loop), which keeps the kernel within its registers.
+        double* s0 = Vg;
+        double* s1 = Vg + P.npad;
+        double* trs = Vg - ENS_GL_STATE;
+        double tr = trs[0], tp1 = trs[2];
+        const double tr_max = trs[1];
+        int shrink = (int)trs[3];
+        double g[NPT];
+        double xsq = 0.0, fsq1 = 0.0;
+        ens_residual(P, A, B, us, forcing, g);
+        __syncthreads();
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) {
+          const int r = threadIdx.x + ET * q;
+          if (r < n) { s0[r] = -x[q]; s1[r] = g[q]; vk[r] = g[q]; }
+          xsq = fma(x[q], x[q], xsq);
+          fsq1 = fma(g[q], g[q], fsq1);
+        }
+        const double nrm_newton = sqrt(blk_sum_all(xsq, red, phase));
+        const double nc = sqrt(blk_sum_all(fsq1, red, phase));  // ||f||_2 at the step's start, as fnorm (same sum, same bits)
+        ens_vjp(P, A, us, vk, g);
+        double gsq = 0.0;
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) gsq = fma(g[q], g[q], gsq);
+        const double l_grad = sqrt(blk_sum_all(gsq, red, phase));
+        // pass 0 (the Newton step leaves the region): ||J du_c||^2 and the dogleg step; pass 1: ||J du||^2 unless known
+        bool have_dJJd = false;
+        double dJJd = 0.0;
+#pragma unroll 1
+        for (int pass = (nrm_newton <= tr) ? 1 : 0; pass < 2 && !have_dJJd; ++pass) {
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) vk[r] = pass == 0 ? -g[q] : s0[r]; }
+          __syncthreads();
+          double wsq = 0.0;
+          {
+            double w[NPT];
+            ens_jvp(P, A, us, vk, w);
+#pragma unroll
+            for (int q = 0; q < NPT; ++q) wsq = fma(w[q], w[q], wsq);
+          }
+          const double jj = blk_sum_all(wsq, red, phase);
+          if (pass == 1) { dJJd = jj; break; }
+          const double quad = jj, d_cauchy = (l_grad * l_grad * l_grad) / quad;
+          if (d_cauchy >= tr) {  // the Cauchy direction cut at the radius: ||J du||^2 is known
+            const double lam = tr / l_grad;
+#pragma unroll
+            for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) s0[r] = lam * -g[q]; }
+            have_dJJd = true;
+            dJJd = lam * lam * quad;
+          } else {  // the dogleg: c1 = (d_cauchy / l_grad) du_c, du = c1 + tau (du_newton - c1) on the sphere
+            const double sc = d_cauchy / l_grad;
+            double aa = 0.0, ab = 0.0;
+#pragma unroll
+            for (int q = 0; q < NPT; ++q) {
+              const int r = threadIdx.x + ET * q;
+              const double c1 = sc * -g[q], c2 = (r < n ? s0[r] : 0.0) - c1;
+              aa = fma(c2, c2, aa);
+              ab = fma(c1, c2, ab);
+            }
+            const double a = blk_sum_all(aa, red, phase), b = 2.0 * blk_sum_all(ab, red, phase);
+            const double c = d_cauchy * d_cauchy - tr * tr;
+            const double aux = fmax(0.0, b * b - 4.0 * a * c);
+            const double tau = (-b + sqrt(aux)) / (2.0 * a);
+#pragma unroll
+            for (int q = 0; q < NPT; ++q) {
+              const int r = threadIdx.x + ET * q;
+              if (r < n) { const double c1 = sc * -g[q]; s0[r] = fma(tau, s0[r] - c1, c1); }
+            }
+          }
+        }
+        // ================= the ratio of actual to predicted decrease (newton.cu trust_region_step; trust_region.jl:396-430) =================
+        double dgp = 0.0, dsq_step = 0.0;
+        {
+          double d[NPT];
+          ens_get(s0, d, n);
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { dgp = fma(d[q], g[q], dgp); dsq_step = fma(d[q], d[q], dsq_step); }
+        }
+        const double dg = blk_sum_all(dgp, red, phase), dun = sqrt(blk_sum_all(dsq_step, red, phase));
+        for (int r = threadIdx.x; r < n; r += ET) vk[r] = us[r] + s0[r];  // u_trial = u + du
+        __syncthreads();
+        double tmx = 0.0, tsq = 0.0;
+        {
+          double ft[NPT];
+          ens_residual(P, A, B, vk, forcing, ft);
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { tmx = fmax(tmx, abs_nf(ft[q])); tsq = fma(ft[q], ft[q], tsq); }
+          ens_put(s0, ft, n);  // du is done with
+        }
+        const double trial_inf = blk_max_all(tmx, red, phase), nt = sqrt(blk_sum_all(tsq, red, phase));
+        const double num = (nt * nt - nc * nc) / 2.0, denom = dg + dJJd / 2.0;
+        const double rho = num / denom;
+        const bool accepted = rho > G.step_thr;
+        // ---- the radius update of the scheme (trust_region.jl:431-499)
+        const int sch = G.scheme;
+        if (sch == B200_TR_SIMPLE) {
+          if (rho < G.shrink_thr) { tr *= G.shrink_fac; ++shrink; }
+          else { shrink = 0; if (rho > G.expand_thr && rho > G.step_thr) tr = G.expand_fac * tr; }
+        } else if (sch == B200_TR_NLSOLVE) {
+          if (rho < G.shrink_thr) { tr *= G.shrink_fac; ++shrink; }
+          else {
+            shrink = 0;
+            if (rho >= G.expand_thr) tr = G.expand_fac * dun;
+            else if (rho >= tp1) { const double e = G.expand_fac * dun; tr = tr < e ? e : tr; }
+          }
+        } else if (sch == B200_TR_NOCEDAL_WRIGHT) {
+          if (rho < G.shrink_thr) { tr = G.shrink_fac * dun; ++shrink; }
+          else { shrink = 0; if (rho > G.expand_thr && fabs(dun - tr) < 1.0e-6 * tr) tr = G.expand_fac * tr; }
+        } else if (sch == B200_TR_HEI) {  // rfunc_adaptive_trust_region :383-391 with (M, beta, g1, g2) = (p1, p2, p3, p4)
+          const double M = tp1, g1 = G.tp3, g2 = G.tp4, beta = G.tp2;
+          const double rf = (rho >= G.shrink_thr) ? (2.0 * (M - 1.0 - g2) * atan(rho - G.shrink_thr) + (1.0 + g2)) / M_PI
+                                                  : (1.0 - g1 - beta) * (exp(rho - G.shrink_thr) + beta / (1.0 - g1 - beta));
+          const double tr_new = rf * dun;
+          if (tr_new < tr) ++shrink; else shrink = 0;
+          tr = tr_new;
+        } else if (sch == B200_TR_YUAN) {
+          if (rho < G.shrink_thr) { tp1 = G.tp2 * tp1; ++shrink; }
+          else { if (rho >= G.expand_thr && 2.0 * dun > tr) tp1 = G.tp3 * tp1; shrink = 0; }
+          // p1 ||J(u_trial)' f(u_trial)||: us and slab column 0 swap (us holds f_trial, column 0 u) for the VJP at the state in vk
+          for (int r = threadIdx.x; r < n; r += ET) { const double t = us[r]; us[r] = s0[r]; s0[r] = t; }
+          __syncthreads();
+          ens_vjp(P, A, vk, us, g);
+          double gsq = 0.0;
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) gsq = fma(g[q], g[q], gsq);
+          tr = tp1 * sqrt(blk_sum_all(gsq, red, phase));
+          for (int r = threadIdx.x; r < n; r += ET) { const double t = us[r]; us[r] = s0[r]; s0[r] = t; }  // and back
+        } else {  // Fan
+          if (rho < G.shrink_thr) { tp1 *= G.tp2; ++shrink; }
+          else { shrink = 0; if (rho > G.expand_thr) tp1 = fmin(tp1 * G.tp3, G.tp4); }
+          tr = tp1 * pow(nt, 0.99);
+        }
+        tr = tr_max < tr ? tr_max : tr;
+        if (accepted) {  // the trial point becomes the iterate
+          for (int r = threadIdx.x; r < n; r += ET) us[r] = vk[r];
+          ens_get(s0, f, n);
+          objective = trial_inf;
+          dsq = dsq_step;  // ||du||_2 = dun again, from the same sum
+        } else {  // u and f stay; GMRES runs again at the same u with the new radius (step norm 0)
+          ens_get(s1, f, n);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) { trs[0] = tr; trs[2] = tp1; trs[3] = (double)shrink; }
+        if (shrink > G.max_shrink) glob_rc = B200_RC_SHRINK_THRESHOLD_EXCEEDED;
+      } else {
+        // ================= BackTracking (newton.cu backtracking; LineSearches.jl, cubic interpolation) =================
+        // phi(a) = ||f(u + a du)||^2 / 2 with the trial state in vk, phi'(0) = <f, J du> by one JVP
+        ens_residual(P, A, B, us, forcing, f);  // not kept in registers through GMRES: the same bits again
+        double d[NPT];
+        double fsq1 = 0.0;
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) { d[q] = -x[q]; fsq1 = fma(f[q], f[q], fsq1); }
+        const double nf0 = sqrt(blk_sum_all(fsq1, red, phase));  // ||f||_2 of the step's start, as fnorm (same sum, same bits)
+        ens_put(vk, d, n);
+        __syncthreads();
+        double dphi0;
+        {
+          double w[NPT];
+          ens_jvp(P, A, us, vk, w);
+          double p = 0.0;
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) p = fma(f[q], w[q], p);
+          dphi0 = blk_sum_all(p, red, phase);
+        }
+        const double phi0 = 0.5 * nf0 * nf0;
+        auto phi = [&](double a) -> double {
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) { const int r = threadIdx.x + ET * q; if (r < n) vk[r] = fma(a, d[q], us[r]); }
+          __syncthreads();
+          double ft[NPT];
+          ens_residual(P, A, B, vk, forcing, ft);
+          double tsq = 0.0;
+#pragma unroll
+          for (int q = 0; q < NPT; ++q) tsq = fma(ft[q], ft[q], tsq);
+          const double t = sqrt(blk_sum_all(tsq, red, phase));  // its barrier also ends every read of vk
+          return 0.5 * t * t;
+        };
+        double a1 = 1.0, a2 = 1.0, phx0 = phi0, phx1 = phi(a1);
+        int itf = 0;
+        while (!isfinite(phx1) && itf < 50) { ++itf; a1 = a2; a2 = a1 / 2.0; phx1 = phi(a2); }
+        int it = 0;
+        while (phx1 > phi0 + G.ls_c1 * a2 * dphi0) {
+          if (++it > G.ls_maxiters) { glob_rc = B200_RC_INTERNAL_LINESEARCH_FAILED; break; }
+          double at;
+          if (it == 1) at = -(dphi0 * a2 * a2) / (2.0 * (phx1 - phi0 - dphi0 * a2));
+          else {
+            const double div = 1.0 / (a1 * a1 * a2 * a2 * (a2 - a1));
+            const double ca = (a1 * a1 * (phx1 - phi0 - dphi0 * a2) - a2 * a2 * (phx0 - phi0 - dphi0 * a1)) * div;
+            const double cb = (-a1 * a1 * a1 * (phx1 - phi0 - dphi0 * a2) + a2 * a2 * a2 * (phx0 - phi0 - dphi0 * a1)) * div;
+            if (fabs(ca) <= 1e-14 * fabs(cb) || ca == 0.0) at = dphi0 / (2.0 * cb);
+            else { const double dd = fmax(cb * cb - 3.0 * ca * dphi0, 0.0); at = (-cb + sqrt(dd)) / (3.0 * ca); }
+          }
+          a1 = a2;
+          const double hi = a2 * G.ls_rho_hi, lo = a2 * G.ls_rho_lo;
+          at = hi < at ? hi : at;
+          a2 = at < lo ? lo : at;
+          phx0 = phx1;
+          phx1 = phi(a2);
+        }
+        // ---- update_u: u += a du with ||a du||_2, fu = f(u)
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) {
+          const int r = threadIdx.x + ET * q;
+          if (r < n) { const double s = a2 * d[q]; us[r] += s; dsq = fma(s, s, dsq); }
+        }
+        __syncthreads();
+        ens_residual(P, A, B, us, forcing, f);
+        fmx = 0.0;
+#pragma unroll
+        for (int q = 0; q < NPT; ++q) fmx = fmax(fmx, abs_nf(f[q]));
+        objective = blk_max_all(fmx, red, phase);
+      }
       const double du_norm = sqrt(blk_sum_all(dsq, red, phase));
       ++nsteps;
       // AbsNorm* termination (termination_conditions.jl:243-336), evaluated redundantly and identically by every thread
@@ -496,6 +824,9 @@ __global__ void __launch_bounds__(ET, 2) ens_newton_kernel(EnsParams P, const do
             if (mx <= P.abstol) { retcode = B200_RC_STALLED; force_stop = 1; }
           }
         }
+      }
+      if constexpr (GL != ENS_GL_NONE) {
+        if (!force_stop && glob_rc != 0) { retcode = glob_rc; force_stop = 1; }
       }
     }
     if (retcode == B200_RC_DEFAULT) retcode = (nsteps >= P.maxiters) ? B200_RC_MAXITERS : B200_RC_SUCCESS;
@@ -550,11 +881,38 @@ int ens_pc(const b200_newton_opts* o) {
   return o->precond == B200_PRECOND_MULTIGRID_LEFT ? ENS_PC_MG_LEFT : o->precond == B200_PRECOND_MULTIGRID_RIGHT ? ENS_PC_MG_RIGHT : ENS_PC_NONE;
 }
 
+int ens_gl(const b200_newton_opts* o) {
+  return o->globalization == B200_GLOBALIZATION_TRUST_REGION ? ENS_GL_TRUST_REGION
+         : o->globalization == B200_GLOBALIZATION_LINESEARCH ? ENS_GL_LINESEARCH : ENS_GL_NONE;
+}
+
+// the instantiations: no preconditioner with any globalisation, multigrid without one
 using EnsKernel = void (*)(EnsParams, const double*, const double*, const double*, const double*, double*, double*, int32_t*, int32_t*,
-                           int32_t*, double*, int*);
-EnsKernel ens_kernel(int pc) {
-  return pc == ENS_PC_MG_LEFT ? ens_newton_kernel<ENS_PC_MG_LEFT> : pc == ENS_PC_MG_RIGHT ? ens_newton_kernel<ENS_PC_MG_RIGHT>
-                                                                                          : ens_newton_kernel<ENS_PC_NONE>;
+                           int32_t*, double*, int*, EnsGlob);
+EnsKernel ens_kernel(int pc, int gl) {
+  if (gl == ENS_GL_TRUST_REGION) return ens_newton_kernel<ENS_PC_NONE, ENS_GL_TRUST_REGION>;
+  if (gl == ENS_GL_LINESEARCH) return ens_newton_kernel<ENS_PC_NONE, ENS_GL_LINESEARCH>;
+  return pc == ENS_PC_MG_LEFT ? ens_newton_kernel<ENS_PC_MG_LEFT, ENS_GL_NONE>
+         : pc == ENS_PC_MG_RIGHT ? ens_newton_kernel<ENS_PC_MG_RIGHT, ENS_GL_NONE>
+                                 : ens_newton_kernel<ENS_PC_NONE, ENS_GL_NONE>;
+}
+
+// the globalisation constants of an option set (the driver's, b200i_tr_params; BackTracking's defaults as in newton.cu)
+EnsGlob ens_glob(const b200_newton_opts* o) {
+  EnsGlob G;
+  memset(&G, 0, sizeof(G));
+  const TrParams p = b200i_tr_params(*o);
+  G.scheme = o->tr_scheme;
+  G.max_shrink = p.max_shrink;
+  G.max_tr = o->tr_max_trust_radius;
+  G.init_tr = o->tr_initial_trust_radius;
+  G.step_thr = p.step_thr; G.shrink_thr = p.shrink_thr; G.expand_thr = p.expand_thr; G.shrink_fac = p.shrink_fac; G.expand_fac = p.expand_fac;
+  G.tp1 = p.tp1; G.tp2 = p.tp2; G.tp3 = p.tp3; G.tp4 = p.tp4;
+  G.ls_c1 = o->ls_c1 > 0 ? o->ls_c1 : 1e-4;
+  G.ls_rho_hi = o->ls_rho_hi > 0 ? o->ls_rho_hi : 0.5;
+  G.ls_rho_lo = o->ls_rho_lo > 0 ? o->ls_rho_lo : 0.1;
+  G.ls_maxiters = o->ls_maxiters > 0 ? o->ls_maxiters : 1000;
+  return G;
 }
 
 int smallest_factor(int n) {
@@ -592,6 +950,7 @@ void ens_params(int32_t N, int32_t nprob, double alpha, const b200_newton_opts* 
   const double dx = 1.0 / (double)(N - 1);
   P.a = alpha / (dx * dx);
   P.slab = (int64_t)(P.kcap + 1) * P.npad + (int64_t)P.kcap * (P.kcap + 1) / 2 + 16;
+  if (o->globalization != B200_GLOBALIZATION_NONE) P.slab += ENS_GL_STATE;
   if (ens_pc(o) != ENS_PC_NONE) {
     P.mg_tab = 2 * P.npad + 4 * (P.kcap + 2) + 100 + 32 + 2 * (ET / 32);
     int off = P.mg_tab + (int)(sizeof(EnsMgLevel) / sizeof(double)) * ENS_MG_MAXLEV;
@@ -627,6 +986,16 @@ int32_t b200i_ens_batched_supported(int32_t N, const b200_newton_opts* o) {
   if (o->term_norm != B200_NORM_INF) return 0;
   if (t != B200_TERM_ABS_NORM && o->term_max_stalled_steps != 0 && o->term_max_stalled_steps != 32) return 0;
   if (o->maxtime > 0.0) return 0;
+  if (o->globalization != B200_GLOBALIZATION_NONE) {  // without a preconditioner (b200_ens_create refuses the combination)
+    if (o->precond != B200_PRECOND_NONE) return 0;
+    if (o->globalization == B200_GLOBALIZATION_TRUST_REGION) {  // the six schemes the C oracle restates; Bastin takes the driver
+      const int s = o->tr_scheme;
+      if (s != B200_TR_SIMPLE && s != B200_TR_NLSOLVE && s != B200_TR_NOCEDAL_WRIGHT && s != B200_TR_HEI && s != B200_TR_YUAN && s != B200_TR_FAN)
+        return 0;
+    } else if (o->globalization != B200_GLOBALIZATION_LINESEARCH) {
+      return 0;
+    }
+  }
   return 1;
 }
 
@@ -635,7 +1004,7 @@ int32_t b200i_ens_batched_ctas_per_sm(b200_ctx* ctx, int32_t N, const b200_newto
   EnsParams P;
   ens_params(N, 1, 1.0, o, &P);
   const size_t smem = ens_smem_bytes(P);
-  const EnsKernel kernel = ens_kernel(ens_pc(o));
+  const EnsKernel kernel = ens_kernel(ens_pc(o), ens_gl(o));
   CUDA_TRY(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int v = 0;
   CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, kernel, ET, smem));
@@ -649,7 +1018,7 @@ int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double 
   EnsParams P;
   ens_params(N, nprob, alpha, o, &P);
   const size_t smem = ens_smem_bytes(P);
-  const EnsKernel kernel = ens_kernel(ens_pc(o));
+  const EnsKernel kernel = ens_kernel(ens_pc(o), ens_gl(o));
   int per_sm = 0;
   B200_TRY(b200i_ens_batched_ctas_per_sm(ctx, N, o, &per_sm));
   if (per_sm < 1) return ctx->fail(B200_ERR_UNSUPPORTED, "ensemble kernel does not fit on an SM", __FILE__, __LINE__);
@@ -677,7 +1046,7 @@ int32_t b200i_ens_batched_solve(b200_ctx* ctx, int32_t N, int32_t nprob, double 
   CUDA_TRY(ctx, cudaMemsetAsync(d_counter, 0, 2 * sizeof(int), ctx->stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(ctx->stream));  // `forcing` is a host temporary
   PLAUNCH(ctx, B200_KID_RESIDENT, 0.0, kernel, grid, ET, smem, P, u0, A, B, (const double*)d_forcing, u_out, resid_inf, retcodes, nsteps,
-          njvp, ws, d_counter);
+          njvp, ws, d_counter, ens_glob(o));
   CHECK_LAUNCH(ctx);
   // trajectories whose Krylov basis outgrew the per-CTA slab (kcap < min(itmax, n)) come back marked B200I_ENS_RC_DEFERRED
   int hits = 0;

@@ -8,7 +8,8 @@
 // Two engines:
 //   * batched (N <= 32): one CTA per trajectory, persistent over a work queue; iterate, residual, Krylov direction and the
 //     Givens recurrence live in shared memory, the Krylov basis streams through a per-CTA slab in HBM/L2; with
-//     Multigrid("left" / "right") the whole V-cycle hierarchy lives in shared memory too (see ens_batched.cu)
+//     Multigrid("left" / "right") the whole V-cycle hierarchy lives in shared memory too; TrustRegion (Dogleg) and
+//     BackTracking without a preconditioner globalise each step inside the same kernel (see ens_batched.cu)
 //   * sequential fallback (any N): the single-system driver of newton.cu, one trajectory after another (block-Jacobi and
 //     every option set the batched kernel does not cover).
 #include "common.cuh"
@@ -63,9 +64,15 @@ int32_t b200_ens_destroy(b200_ensemble* e) {
 int32_t b200_ens_create(b200_ctx* ctx, int32_t N, int32_t nprob_local, double alpha, const b200_newton_opts* opts, b200_ensemble** out) {
   B200_DEVICE_GUARD(ctx);
   B200_REQUIRE(ctx, N >= 3 && nprob_local > 0 && opts && out, "ens_create: bad arguments");
-  B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_GMRES && opts->globalization == B200_GLOBALIZATION_NONE && opts->descent == B200_DESCENT_NEWTON,
-               "ensemble: only matrix-free NewtonRaphson(linsolve = GMRES) trajectories are batched");
+  B200_REQUIRE(ctx, opts->linsolve == B200_LINSOLVE_GMRES && opts->descent == B200_DESCENT_NEWTON,
+               "ensemble: only matrix-free Newton(linsolve = GMRES) trajectories are batched: NewtonRaphson, with or without "
+               "linesearch = BackTracking(), or TrustRegion");
+  B200_REQUIRE(ctx, opts->globalization == B200_GLOBALIZATION_NONE || opts->globalization == B200_GLOBALIZATION_TRUST_REGION ||
+                        opts->globalization == B200_GLOBALIZATION_LINESEARCH,
+               "ensemble: unknown globalization");
   const int32_t pc = opts->precond;
+  B200_REQUIRE(ctx, opts->globalization == B200_GLOBALIZATION_NONE || pc == B200_PRECOND_NONE,
+               "ensemble: a globalised ensemble (TrustRegion, BackTracking) takes no preconditioner");
   B200_REQUIRE(ctx, pc != B200_PRECOND_ILU0_LEFT && pc != B200_PRECOND_ILU0_RIGHT && pc != B200_PRECOND_AMG_LEFT && pc != B200_PRECOND_AMG_RIGHT &&
                         pc != B200_PRECOND_SA_AMG_LEFT && pc != B200_PRECOND_SA_AMG_RIGHT,
                "ensemble: ILU0 and AMG precondition the assembled sparse Jacobian, and ensemble trajectories are matrix-free: use "

@@ -30,13 +30,6 @@ struct TermCache {  // NonlinearTerminationModeCache (termination_conditions.jl:
 struct TermQuant {
   double f_inf, f_norm, sum_norm, rel_viol;  // ||f||_inf ; internalnorm(f) ; internalnorm(f + u) ; #{ |f_i| > reltol |u_i + f_i| }
 };
-// The radius update scheme's constants (get_parameters, trust_region.jl:348-381): thresholds, factors and the shrink limit
-// hold for the solver's life; tp1..tp4 are the initial scheme parameters, restored by every reinit (Yuan and Fan mutate p1).
-struct TrParams {
-  double step_thr, shrink_thr, expand_thr, shrink_fac, expand_fac;
-  int max_shrink;
-  double tp1, tp2, tp3, tp4;
-};
 }  // namespace
 
 struct b200_newton {
@@ -183,23 +176,6 @@ int32_t dev_vecs(b200_newton* nw, std::initializer_list<double**> ps) {
   return B200_OK;
 }
 
-TrParams tr_params(const b200_newton_opts& o) {
-  const int sch = o.tr_scheme;
-  TrParams p;
-  p.step_thr = o.tr_step_threshold > 0 ? o.tr_step_threshold : (sch == B200_TR_HEI ? 0.0 : sch == B200_TR_YUAN ? 1.0 / 1000 : sch == B200_TR_BASTIN ? 1.0 / 20 : 1.0 / 10000);
-  p.shrink_thr = o.tr_shrink_threshold > 0 ? o.tr_shrink_threshold : (sch == B200_TR_HEI ? 0.0 : (sch == B200_TR_NLSOLVE || sch == B200_TR_BASTIN) ? 1.0 / 20 : 0.25);
-  p.expand_thr = o.tr_expand_threshold > 0 ? o.tr_expand_threshold : ((sch == B200_TR_NLSOLVE || sch == B200_TR_BASTIN) ? 0.9 : sch == B200_TR_HEI ? 0.0 : 0.75);
-  p.shrink_fac = o.tr_shrink_factor > 0 ? o.tr_shrink_factor : (sch == B200_TR_NLSOLVE ? 0.5 : sch == B200_TR_HEI ? 0.0 : sch == B200_TR_BASTIN ? 1.0 / 20 : 0.25);
-  p.expand_fac = o.tr_expand_factor > 0 ? o.tr_expand_factor : 2.0;
-  p.max_shrink = o.max_shrink_times > 0 ? o.max_shrink_times : 32;
-  p.tp1 = p.tp2 = p.tp3 = p.tp4 = 0.0;
-  if (sch == B200_TR_NLSOLVE) { p.tp1 = 0.5; }
-  else if (sch == B200_TR_HEI) { p.tp1 = 5.0; p.tp2 = 0.1; p.tp3 = 0.15; p.tp4 = 0.15; }
-  else if (sch == B200_TR_YUAN) { p.tp1 = 2.0; p.tp2 = 1.0 / 6; p.tp3 = 6.0; }
-  else if (sch == B200_TR_FAN) { p.tp1 = 0.1; p.tp2 = 0.25; p.tp3 = 12.0; p.tp4 = 1.0e18; }
-  else if (sch == B200_TR_BASTIN) { p.tp1 = 2.5; p.tp2 = 0.25; }
-  return p;
-}
 }  // namespace
 
 extern "C" {
@@ -352,7 +328,7 @@ int32_t b200_newton_create(b200_problem* prob, const b200_newton_opts* opts, b20
   nw->abstol = opts->abstol > 0 ? opts->abstol : 3.0e-13;  // common_defaults.jl:44-48
   nw->reltol = opts->reltol > 0 ? opts->reltol : 3.0e-13;
   nw->maxiters = opts->maxiters > 0 ? opts->maxiters : 1000;
-  nw->trp = tr_params(*opts);
+  nw->trp = b200i_tr_params(*opts);
   const int32_t s = newton_setup(nw);
   if (s != B200_OK) { b200_newton_destroy(nw); return s; }
   *out = nw;
